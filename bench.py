@@ -2,7 +2,7 @@
 """Benchmark of the hot path (contract in the task statement, tier rule 4/5).
 
 N = 1 -- BASELINE.json configs[1], "MPS norm/expectation contraction L=200
-chi=1024 fp64 on 1xB200".  A *step* is one full contraction <psi|psi> of a
+chi=1024 fp64 on 1 GPU".  A *step* is one full contraction <psi|psi> of a
 synthetic random MPS (L=200, bond 1024, d=2, fp64): 400 launches of the
 pairwise contraction kernel, 1.55 TFLOP of algorithmic work (sum over sites
 of 2 l l d r + 2 l d r r).  `value` is device-resident throughput, `e2e` the
@@ -26,6 +26,14 @@ state spends 30-100) on a = b = 1024, d = 2, w = 5: 24 x 86.7 GFLOP.
 grows ("scaling": "strong").
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+                  [--dump-outputs DIR]
+
+`--dump-outputs DIR` writes what the timed path returned in its last timed
+step as DIR/<name>.npy (float64): N = 1 the final environment of the norm
+contraction (`mps_norm_env`, shape (1, 1)); N > 1 the Ritz value (`theta`) and
+each rank's slab of the Ritz vector (`x_rank<r>`, 32 MiB / N).  The inputs are
+generated from fixed seeds, so two builds run with the same arguments can be
+compared output for output.
 
 `--impl reference` times the reference's own CPU path for the same config
 (the numpy/OpenBLAS restatement in oracle/ -- the reference is pure Python +
@@ -250,41 +258,6 @@ def run_reference(args, rank, world):
     print(json.dumps(line), flush=True)
 
 
-# ------------------------------------------------------- profile summaries ---
-_UNIT = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-
-
-def profile_traffic(path, kernel_substr=None):
-    """dram read + write bytes per launch from a committed `ncu --set full`
-    summary (profiles/*.txt as written by tools/summarize_profiles.py)."""
-    rd = wr = None
-    try:
-        for ln in open(path):
-            for key in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                if ln.startswith(key + " ["):
-                    unit = ln[len(key) + 2:ln.index("]")]
-                    vals = [float(x) * _UNIT.get(unit, 1.0)
-                            for x in ln.split(":", 1)[1].split("|")]
-                    if key.endswith("read.sum"):
-                        rd = vals
-                    else:
-                        wr = vals
-        if rd and wr:
-            return float(np.mean(rd) + np.mean(wr))
-    except Exception:
-        pass
-    return None
-
-
-def newest_profile(prefixes):
-    pdir = os.path.join(ROOT, "profiles")
-    for pre in prefixes:
-        p = os.path.join(pdir, pre)
-        if os.path.exists(p):
-            return p
-    return None
-
-
 # ---------------------------------------------------------------- GPU arm ---
 def build_unit_problem(qb, dev):
     """chi=1024 environments of the centre bond of a random L=24 Heisenberg
@@ -306,7 +279,8 @@ def build_unit_problem(qb, dev):
 
 
 def run_unit(qb, shard, prob, steps, warmup, barrier, events=True):
-    """Time `steps` eigensolve cycles of UNIT_MATVECS matvecs each."""
+    """Time `steps` eigensolve cycles of UNIT_MATVECS matvecs each; returns
+    (ms per step, Ritz value, Ritz vector of the last step, operator)."""
     import torch
     from quimb_b200.dmrg import EffHam2, ShardedEffHam2
     Lenv, W1, W2, Renv, v0, dims = prob
@@ -335,7 +309,7 @@ def run_unit(qb, shard, prob, steps, warmup, barrier, events=True):
     assert nmv == UNIT_MATVECS, nmv
     if shard is not None:
         shard.check()           # a peer-memory kernel that gave up waiting would show here
-    return ev0.elapsed_time(ev1) / steps, theta, H
+    return ev0.elapsed_time(ev1) / steps, theta, x, H
 
 
 def time_exchange(shard, prob, reps=20):
@@ -368,6 +342,8 @@ def main():
     ap.add_argument("--no-dmrg", action="store_true")
     ap.add_argument("--exchange", default=os.environ.get("QB_EXCHANGE", "auto"),
                     help="N>1: auto | p2p | nccl")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -429,7 +405,12 @@ def bench_sharded(args, qb, _lib, dist, dev, rank, local_rank, world, barrier, m
     if rank == 0:
         sampler.start()
     n0 = _lib.launch_count()
-    ms, theta, H = run_unit(qb, shard, prob, args.steps, args.warmup, barrier)
+    ms, theta, x, H = run_unit(qb, shard, prob, args.steps, args.warmup, barrier)
+    if args.dump_outputs:
+        outs = {f"x_rank{rank}": x.to_numpy()}
+        if rank == 0:
+            outs["theta"] = np.asarray(theta)
+        dump_outputs(args.dump_outputs, outs)
     launches = _lib.launch_count() - n0
     clocks = sampler.stop() if rank == 0 else None
     ms_max = max_over_ranks(ms)
@@ -441,8 +422,8 @@ def bench_sharded(args, qb, _lib, dist, dev, rank, local_rank, world, barrier, m
     # N=1 point of the strong-scaling curve, measured next to the N-rank run
     single_ms = None
     if rank == 0:
-        single_ms, theta1, _ = run_unit(qb, None, prob, max(2, args.steps // 2), 2,
-                                        torch.cuda.synchronize)
+        single_ms, theta1, _, _ = run_unit(qb, None, prob, max(2, args.steps // 2), 2,
+                                           torch.cuda.synchronize)
         assert abs(theta1 - theta) <= 1e-9 * abs(theta), (theta1, theta)
     barrier()
 
@@ -571,6 +552,8 @@ def bench_mps_norm(args, qb, _lib, dev, barrier):
     ms_max = ev0.elapsed_time(ev1) / args.steps
     value = flops / (ms_max * 1e-3) / 1e12
     norm2 = float(out.reshape(()).item())
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"mps_norm_env": out.to_numpy()})
 
     # dominant kernel: the full-size (chi x chi.d x chi) contraction launches
     big = [(a.elapsed_time(b), fl) for a, b, fl, l, r in records if l == CHI and r == CHI]
@@ -626,29 +609,18 @@ def bench_mps_norm(args, qb, _lib, dev, barrier):
 
     # ---- roofline denominators --------------------------------------------
     peak = dmma_peak(_lib)
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    prof = newest_profile(["r02_contract_kernel_ncu_full.txt", "r01_contract_kernel_ncu_full.txt"])
-    traffic = profile_traffic(prof) if prof else None
     roofline = {
         "bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
-        "frac": achieved / peak if peak else None, "traffic": traffic,
-        "traffic_source": (os.path.relpath(prof, ROOT) if prof else None),
+        "frac": achieved / peak if peak else None, "traffic": None,
         "algorithmic_bytes_per_launch": 8 * (CHI * CHI + 2 * CHI * PHYS * CHI),
         "kernel": "contract_f64_streamk_kernel<128,128,32> (DMMA fp64, persistent stream-K)",
-        "peak_source": "fp64 DMMA issue-rate microbenchmark measured live on this GPU "
-                       "(tcgen05 has no f64 kind; MEASURED_PEAKS.json holds bf16 only)",
+        "peak_source": "fp64 DMMA issue-rate microbenchmark measured live on this GPU",
         "flops_per_launch": k_fl, "ms_per_launch": k_ms,
-        "bf16_peak_measured": peaks.get("bf16_tflops"),
-        "frac_of_bf16_measured": (achieved / peaks["bf16_tflops"]) if peaks.get("bf16_tflops") else None,
     }
 
     # ---- the unit the multi-GPU line shards, unsharded on this GPU -----------
     prob = build_unit_problem(qb, dev)
-    unit_ms, theta, H = run_unit(qb, None, prob, max(2, args.steps // 2), 2, barrier)
+    unit_ms, theta, _, H = run_unit(qb, None, prob, max(2, args.steps // 2), 2, barrier)
     unit_flops = UNIT_MATVECS * matvec_flops()
     shard_unit = {"workload": config_shard(1)["workload"], "ms_per_step": unit_ms,
                   "tflops": unit_flops / (unit_ms * 1e-3) / 1e12,
@@ -675,6 +647,14 @@ def bench_mps_norm(args, qb, _lib, dev, barrier):
         "roofline": roofline, "cpu_baseline": cpu, "shard_unit": shard_unit, "dmrg": dmrg,
         "check": {"norm2": norm2},
     }
+
+
+def dump_outputs(dirname, arrays):
+    """Write each array as dirname/<name>.npy in float64 (complex is not
+    produced by these workloads)."""
+    os.makedirs(dirname, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(dirname, f"{name}.npy"), np.asarray(a, dtype=np.float64))
 
 
 def bench_dmrg_updates(qb):
@@ -712,8 +692,7 @@ def bench_dmrg_updates(qb):
     return {"s_per_update_chi1024": per, "updates_timed": len(times),
             "matvecs_per_update": float(np.mean(nmv)),
             "sweep_s_L100_extrapolated": per * 79 + per * 0.25 * 20,
-            "note": "first right sweep from a random state (hardest local problems); "
-                    "a measured full L=100 sweep is in profiles/",
+            "note": "first right sweep from a random state (hardest local problems)",
             "energy_after": energies[-1]}
 
 

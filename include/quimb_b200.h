@@ -1,5 +1,5 @@
 /*
- * quimb_b200 -- C ABI of the B200-native tensor-network contraction engine.
+ * quimb_b200 -- C ABI of the H100-native tensor-network contraction engine.
  *
  * This header is the drop-in boundary.  Every entry point replaces one
  * library call that quimb's hot path bottoms out in (all reference citations
@@ -92,11 +92,11 @@ enum {
 enum {
   QB_ENGINE_AUTO = 0, /* heuristic                                    */
   QB_ENGINE_DMMA = 1, /* native fp64 tensor-core path (DMMA)          */
-  QB_ENGINE_OZAKI = 2, /* tcgen05 int8 error-free-split path (fp64)    */
+  QB_ENGINE_OZAKI = 2, /* int8 tensor-core (wgmma) error-free-split path */
   QB_ENGINE_STREAM = 3, /* HBM-bound streaming path for small-operator
                          * steps (N <= 16 and K <= 16 after mode grouping:
                          * gate application); other shapes take the DMMA
-                         * path.  Opt-in until timed on a B200.          */
+                         * path.  Opt-in: not timed on the H100.        */
   /* OR-able flag: the caller guarantees that bytes [0, 1024) of `workspace`
    * (the stream-K flag words) were zero before its first use and are written
    * by this library only -- which always leaves them zero again -- so the

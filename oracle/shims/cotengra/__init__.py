@@ -135,7 +135,7 @@ def _dispatched_contract(arrays, inputs, output, path, size_dict, strip_exponent
     node is ``do("tensordot")`` (+ ``do("transpose")``) when the pair is a
     pure tensordot and ``do("einsum")`` otherwise, dispatched by autoray on
     the array type (or ``backend``).  Used when the unmodified reference is
-    driven with device arrays as ``Tensor._data`` (tests/test_dropin_reference_cpu.py)."""
+    driven with device arrays as ``Tensor._data``."""
     from autoray import do
     arrays = list(arrays)
     terms = [tuple(t) for t in inputs]

@@ -1,4 +1,4 @@
-"""quimb_b200 -- a B200-native array backend for quimb's hot path.
+"""quimb_b200 -- an H100-native array backend for quimb's hot path.
 
 The module *is* the backend: arrays are :class:`quimb_b200.Array`, so
 ``autoray.infer_backend(x) == "quimb_b200"`` and
@@ -10,7 +10,7 @@ fused overrides of quimb's composed split drivers (``svd_truncated``,
 ``qr_stabilized``, ``fuse`` ...), exactly as quimb itself does for its numpy
 backend (quimb/tensor/decomp.py:1058, :2198).
 
-All arithmetic on the hot path runs in hand-written sm_100a CUDA kernels
+All arithmetic on the hot path runs in hand-written sm_90a CUDA kernels
 behind a C ABI (``include/quimb_b200.h``); there is no CPU fallback.
 """
 

@@ -71,7 +71,7 @@ def contract_pair(a, la, b, lb, lc, conj_a=False, conj_b=False, out=None,
     if len(la) != a.dim() or len(lb) != b.dim():
         raise ValueError("label count does not match operand rank")
     if a.dtype in _WIDE and not _native_single(a, la, b, lb, lc, out, engine):
-        # single precision below the tcgen05 engine's tile minimum (or with
+        # single precision below the int8 engine's tile minimum (or with
         # batch modes): widen exactly, contract in fp64, round once
         wide = _WIDE[a.dtype]
         wout = None if out is None else convert(out, wide)
@@ -132,7 +132,7 @@ _NO_NATIVE_SINGLE = -101
 
 def _native_single(a, la, b, lb, lc, out, engine):
     """True when the library takes this float32 / complex64 contraction on its
-    native engine (tcgen05, 4 int8 slices, float epilogue -- csrc/ozaki_tc.cu);
+    native engine (int8 wgmma, 4 slices, float epilogue -- csrc/ozaki_tc.cu);
     decided by the library's own planner, so the rule lives in one place."""
     ext = {}
     for t, ls in ((a, la), (b, lb)):

@@ -26,7 +26,7 @@ int sm_count() {
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) !=
             cudaSuccess)
-      n = 148;
+      n = 132;  // H100 SXM
   }
   return n;
 }
@@ -71,14 +71,14 @@ int gemm_f64(const double *A, int64_t a_rs, int64_t a_cs, const double *B,
 
 static bool is_single(int dt) { return dt == QB_F32 || dt == QB_C64; }
 
-// f64 / c128: every engine.  f32 / c64: the tcgen05 engine only (4 int8
+// f64 / c128: every engine.  f32 / c64: the int8 engine only (4 int8
 // slices, float epilogue); shapes below its tile minimum are refused with
 // QB_NO_NATIVE_SINGLE and the host layer widens them instead.
 constexpr int QB_NO_NATIVE_SINGLE = -101;
 static int check_device_dtype(const PairPlan &plan) {
   if (is_single(plan.dtype) && !(plan.empty_out || plan.zero_fill) && !ozaki_eligible(plan)) {
     set_error("single-precision contraction M=%lld N=%lld K=%lld batch=%lld is below the "
-              "tcgen05 engine's minimum (M >= 128, N >= 64, K >= 128 real units, no "
+              "int8 engine's minimum (M >= 128, N >= 64, K >= 128 real units, no "
               "batch modes): widen it", (long long)plan.p.M, (long long)plan.p.N,
               (long long)plan.p.K, (long long)plan.p.nbatch);
     return QB_NO_NATIVE_SINGLE;
@@ -102,18 +102,13 @@ static int env_engine() {
   }();
   return v;
 }
-// float64 GEMM-shaped contractions from this many flops up take the tcgen05
-// engine under QB_ENGINE_AUTO: measured on a B200 (profiles/r02_matvec_probe.json)
-// it wins at 4096^3 (41.4 vs 32.9 TFLOP/s for the DMMA kernel, cuBLAS dgemm 35.4)
-// and loses at 2048^3 (28.2 vs 31.2) and on the 4.3e10-flop DMRG GEMMs (within
-// +-9 %); BASELINE configs[0] (two rank-4 chi=64 tensors = 4096^3) is above it.
-constexpr double kOzakiAutoFlops = 1.0e11;
+// float64 / complex128 take the int8 engine only on request: on the H100 its
+// 36 slice products bound it to ~55 TFLOP/s fp64-equivalent (1979 int8 TOPS /
+// 36), below the 67 TFLOP/s DMMA peak at every size, and it was measured
+// slower than the DMMA kernel at 2048^3 and 4096^3 (DESIGN.md section 4.6).
 static bool want_ozaki(int engine, const PairPlan &plan) {
   if (is_single(plan.dtype)) return ozaki_eligible(plan);   // the only native engine
   if (engine == QB_ENGINE_AUTO) engine = env_engine();
-  if (engine == QB_ENGINE_AUTO && plan.dtype == QB_F64 &&
-      2.0 * (double)plan.p.M * (double)plan.p.N * (double)plan.p.K >= kOzakiAutoFlops)
-    return ozaki_eligible(plan);
   return engine == QB_ENGINE_OZAKI && ozaki_eligible(plan);
 }
 // streaming engine (contract_stream.cu): small-operator steps, N, K <= 16

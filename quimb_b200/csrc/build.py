@@ -1,8 +1,7 @@
-"""Build libquimb_b200.so in-tree with nvcc for sm_100a.
+"""Build libquimb_b200.so in-tree with nvcc for sm_90a (H100).
 
 Usage: python -m quimb_b200.csrc.build [--force] [--verbose]
-The shared object lands next to the sources (git-ignored, but shipped to the
-GPU box by gpurun).
+The shared object lands next to the sources (git-ignored build product).
 """
 
 import hashlib
@@ -23,8 +22,10 @@ HEADERS = sorted(os.path.basename(p) for p in glob.glob(os.path.join(HERE, "*.h"
 LIB = os.path.join(HERE, "libquimb_b200.so")
 STAMP = os.path.join(HERE, ".build_stamp")
 
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *ARCH,
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "-cudart", "static",
@@ -81,8 +82,7 @@ def build(force=False, verbose=False):
     # link next to the target and rename: the library is replaced atomically
     # (a snapshot of the tree never sees a half-written .so)
     tmp = LIB + ".tmp"
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a",
-           "-cudart", "static", "-o", tmp, *objs]
+    cmd = [nvcc, "-shared", *ARCH, "-cudart", "static", "-o", tmp, *objs]
     subprocess.run(cmd, check=True)
     os.replace(tmp, LIB)
     with open(STAMP, "w") as fh:

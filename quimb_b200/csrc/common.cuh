@@ -1,4 +1,4 @@
-// Shared helpers for the quimb_b200 CUDA sources (sm_100a only).
+// Shared helpers for the quimb_b200 CUDA sources (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -81,7 +81,7 @@ __device__ __forceinline__ void cp_async_wait() {
 }
 
 // D(16x8) += A(16x8, row) * B(8x8, col) in fp64 on the tensor cores
-// (SASS: 4 x DMMA.8x8x4 on sm_100a).  Fragment ownership (g = lane/4,
+// (one DMMA on sm_90a).  Fragment ownership (g = lane/4,
 // t = lane%4):  a0:(g,t) a1:(g+8,t) a2:(g,t+4) a3:(g+8,t+4);
 // b0:(k=t,n=g) b1:(k=t+4,n=g);  c0:(g,2t) c1:(g,2t+1) c2:(g+8,2t) c3:(g+8,2t+1)
 __device__ __forceinline__ void dmma_16x8x8(double (&c)[4], const double (&a)[4],

@@ -1,4 +1,4 @@
-// Pairwise tensor contraction on the fp64 tensor cores (DMMA) of sm_100a.
+// Pairwise tensor contraction on the fp64 tensor cores (DMMA) of sm_90a.
 //
 //   C[m, n, batch] = sum_k op(A)[m, k, batch] * op(B)[k, n, batch]
 //
@@ -473,7 +473,7 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
 
 template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
           bool CPLX, int LA = -1, int LB = -1, int DBG = 0>
-__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32)
+__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
     contract_f64_kernel(const __grid_constant__ ContractParams p) {
   const int64_t Kh = CPLX ? 2 * p.K : p.K;
   const int ks = blockIdx.z;
@@ -493,7 +493,7 @@ __global__ void __launch_bounds__(WARPS_M *WARPS_N * 32)
 // adds them in a fixed order and runs the normal epilogue.
 template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
           bool CPLX, int LA = -1, int LB = -1>
-__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32)
+__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
     contract_f64_streamk_kernel(const __grid_constant__ ContractParams p) {
   const int64_t Kh = CPLX ? 2 * p.K : p.K;
   const int64_t nkbT = (Kh + BK - 1) / BK;
@@ -701,7 +701,7 @@ static int launch_contract_t(const PairPlan &plan, cudaStream_t st) {
   if (rc) return rc;
   if (p.splitk > 1) {
     int64_t total = p.M * p.N * p.nbatch * (CPLX ? 2 : 1);
-    int blocks = (int)std::min<int64_t>((total + 255) / 256, 148 * 8);
+    int blocks = (int)std::min<int64_t>((total + 255) / 256, (int64_t)sm_count() * 8);
     splitk_reduce_f64_kernel<CPLX><<<blocks, 256, 0, st>>>(p);
     QB_LAUNCH_CHECK();
   }

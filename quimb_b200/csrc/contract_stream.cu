@@ -17,7 +17,8 @@
 // calls it).
 //
 // Status: selected only on explicit request (QB_ENGINE_STREAM, or
-// QB_ENGINE=stream in the environment) until it has been timed on a B200.
+// QB_ENGINE=stream in the environment): it has not been timed against the
+// DMMA path on the H100.
 #include <cuda_runtime.h>
 
 #include "internal.h"

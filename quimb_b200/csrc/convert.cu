@@ -2,7 +2,7 @@
 // by widening them to f64 / c128 (exact), running the fp64 engines and
 // rounding the result once -- every intermediate product/sum is carried in
 // fp64, so results are at least as accurate as the reference's fp32 path.
-// A native TF32x3 tcgen05 engine is the planned replacement.
+// Shapes above its tile minimum take the native int8 engine (ozaki_tc.cu).
 #include "common.cuh"
 
 namespace qb {

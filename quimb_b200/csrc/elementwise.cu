@@ -329,7 +329,7 @@ int launch_fill_zero(const qb_tensor_t *C, cudaStream_t st) {
       d.shape[i] = C->shape[i];
       d.stride[i] = C->stride[i] * epr;
     }
-    int blocks = (int)std::min<int64_t>((n + 255) / 256, 148 * 8);
+    int blocks = (int)std::min<int64_t>((n + 255) / 256, (int64_t)sm_count() * 8);
     fill_zero_strided_kernel<<<blocks, 256, 0, st>>>(static_cast<double *>(C->ptr), d, n,
                                                      epr, real_bytes);
     QB_LAUNCH_CHECK();
@@ -337,7 +337,7 @@ int launch_fill_zero(const qb_tensor_t *C, cudaStream_t st) {
   }
   int64_t n16 = bytes / 16;
   int tail = (int)(bytes - n16 * 16);
-  int blocks = (int)std::min<int64_t>((n16 + 255) / 256 + 1, 148 * 8);
+  int blocks = (int)std::min<int64_t>((n16 + 255) / 256 + 1, (int64_t)sm_count() * 8);
   fill_zero_kernel<<<blocks, 256, 0, st>>>(C->ptr, n16, n16 * 16, tail);
   QB_LAUNCH_CHECK();
   return 0;

@@ -9,7 +9,7 @@ int launch_contract_f64(const PairPlan &plan, cudaStream_t st);
 int launch_contract_c128(const PairPlan &plan, cudaStream_t st);
 int launch_fill_zero(const qb_tensor_t *C, cudaStream_t st);
 
-// tcgen05 int8 error-free-split engine (ozaki_tc.cu)
+// int8 tensor-core (wgmma) error-free-split engine (ozaki_tc.cu)
 bool ozaki_eligible(const PairPlan &plan);
 int64_t ozaki_workspace_bytes(const PairPlan &plan);
 int launch_contract_ozaki(const PairPlan &plan, void *workspace, cudaStream_t st);

@@ -15,7 +15,7 @@
 //                  tiles, cyclic Jacobi eigen-solve of the 2b x 2b Gram in
 //                  shared memory, rotation applied to the columns of the
 //                  working matrix and of V.  The working set (n x n twice)
-//                  is L2 resident on B200 (126 MB) up to n = 2048.
+//                  is 64 MB at n = 2048 (the H100's L2 holds 50 MB).
 //   qb_svals_to_keep <- _compute_number_svals_to_keep_numba + renorm factor
 //                  (decomp.py:901-965), host side, bit-for-bit the same
 //                  summation order as the reference.
@@ -362,13 +362,14 @@ int qr_f64(int64_t m, int64_t n, const double *X, double *Q, double *R,
                                 cudaMemcpyDeviceToDevice, st));
   int rc;
   int64_t po = 0;
-  // Aggregation pays when the trailing matrix does not stay in L2 (tall
-  // matrices: 16384 x 2048 went 179 -> 60 ms); for an L2-resident matrix the
-  // extra Gram GEMM + triangular inverse per outer panel cost more than the
-  // narrower updates save (2048 x 1024: 6.9 -> 8.7 ms), so there every inner
-  // panel is its own outer panel and its T is used as it comes.
-  // (measured: 2048^2 = 32 MiB 13.8 vs 17.6 ms without / with aggregation,
-  // 8192 x 1024 = 64 MiB 19.6 vs 15.6 ms, 16384 x 2048 179 vs 60 ms)
+  // Aggregation pays when the trailing matrix does not stay in L2; for an
+  // L2-resident matrix the extra Gram GEMM + triangular inverse per outer
+  // panel cost more than the narrower updates save, so there every inner
+  // panel is its own outer panel and its T is used as it comes.  Measured on
+  // an H100 SXM at a 400 W power limit, Q and R, without / with aggregation:
+  // 2048 x 1024 (16 MiB) 9.3 / 11.2 ms, 2048^2 (32 MiB) 19.7 / 22.7 ms,
+  // 3072 x 2048 (48 MiB) 25.5 / 27.1 ms, 4096 x 2048 (64 MiB) 31.2 / 31.4 ms,
+  // 4096^2 (128 MiB) 66.3 / 60.3 ms.
   const int64_t nbo = (m > 4096 || m * n * 8 > (int64_t)48 << 20) ? QR_NBO : nb;
   for (int64_t j0 = 0; j0 < k; j0 += nbo, ++po) {
     const int w = (int)std::min<int64_t>(nbo, k - j0);   // outer panel width

@@ -1,7 +1,7 @@
-// fp64 pairwise contraction on the 5th-generation tensor cores (tcgen05).
+// fp64 pairwise contraction on the int8 tensor cores (Hopper wgmma).
 //
-// tcgen05.mma has no f64 kind, so large real-fp64 contractions are run as an
-// ERROR-FREE integer decomposition (Ozaki scheme) on kind::i8:
+// The tensor cores' fp64 rate is far below their int8 rate, so large real-fp64
+// contractions can run as an ERROR-FREE integer decomposition (Ozaki scheme):
 //
 //   A[m,k] = 2^eA[m] * sum_p qA_p[m,k] 2^-(6+7p),   qA_p in [-64, 64] (int8)
 //   B[k,n] = 2^eB[n] * sum_q qB_q[k,n] 2^-(6+7q)
@@ -19,27 +19,27 @@
 //                            planes [S][rows][K]; the INDEX PERMUTATION of the
 //                            contraction is folded into this gather, so the
 //                            GEMM kernel sees canonical operands  (HBM bound)
-//   3. ozaki_gemm_kernel     128 x 64 output tile per CTA.  Warp-specialised:
-//        warp 0  TMA producer: cp.async.bulk.tensor (SWIZZLE_128B) of the S
-//                B-slice tiles of a k-block (double buffered) and of the A
-//                slice tiles through a 4-slot ring, mbarrier full/empty;
-//        warp 1  one thread issues tcgen05.mma.kind::i8 (M=128,N=64,K=32):
+//   3. ozaki_gemm_kernel     128 x BN output tile per CTA, 3 warpgroups:
+//        warpgroup 0  TMA producer (one thread, registers handed to the
+//                consumers with setmaxnreg): cp.async.bulk.tensor
+//                (SWIZZLE_128B) of the S B-slice tiles of a k-block (double
+//                buffered) and of the A slice tiles through a 4-slot ring,
+//                mbarrier full/empty;
+//        warpgroups 1-2  64 rows each: wgmma.mma_async m64nBNk32 s8.s8.s32,
 //                for p: for q <= S-1-p: acc[p+q] += A_p B_q; the S
-//                anti-diagonal accumulators (S x 64 columns x 128 lanes of
-//                int32) live in TMEM (all 512 columns); tcgen05.commit
-//                releases smem slots and finally signals the epilogue;
-//        warps 2-5  epilogue: tcgen05.ld the S accumulators, combine them
-//                in fp64 with exact power-of-two weights, apply the row /
-//                column scales and alpha/beta, scatter to the strided C
-//                (output permutation folded into the store).
+//                anti-diagonal accumulators live in registers (S x BN/2 per
+//                thread); then the epilogue combines them in fp64 with exact
+//                power-of-two weights, applies the row / column scales and
+//                alpha/beta and scatters to the strided C (output
+//                permutation folded into the store).
 //
-// Round 2: the same engine serves all four dtypes natively.
-//   * float32 / complex64 (BASELINE configs[4]: PEPS boundary contraction):
-//     S = 4 slices (6 + 7*3 = 27 bits below the row maximum, finer than the
-//     24-bit significand), 10 slice products, 128 x 128 output tiles (4
-//     accumulators x 128 TMEM columns); the split kernel reads the strided
-//     single-precision operand directly and the epilogue rounds once to
-//     float -- no widening passes through HBM.
+// The same engine serves all four dtypes natively.
+//   * float32 / complex64 (PEPS boundary contraction): S = 4 slices (6 + 7*3
+//     = 27 bits below the row maximum, finer than the 24-bit significand),
+//     10 slice products, 128 x 64 output tiles; the split kernel reads the
+//     strided single-precision operand directly and the epilogue rounds once
+//     to float -- no widening passes through HBM.  float64: S = 8, 36 slice
+//     products, 128 x 32 tiles.
 //   * complex64 / complex128: the real GEMM of the embedding
 //       A_e[m, 2k+c] = (re, im)(A[m,k]),   B_e[2k+c, 2n+d] = [[re, im], [-im, re]]
 //     (C_e[m, 2n+d] is the interleaved storage of complex C); the embedding is
@@ -54,12 +54,14 @@
 
 namespace qb {
 
-constexpr int OZ_BM = 128;     // tile rows (TMEM lanes)
+constexpr int OZ_BM = 128;     // tile rows (2 consumer warpgroups x 64)
 constexpr int OZ_BK = 128;     // bytes (= int8 elements) of K per slice tile
-constexpr int OZ_MAXS = 8;     // max slices: S * BN <= 512 TMEM columns
+constexpr int OZ_MAXS = 8;     // max slices, double: 8 x 32 columns of accumulators
+constexpr int OZ_MAXS_SINGLE = 4;  // max slices, single: 4 x 64 columns
+constexpr int OZ_BN_DOUBLE = 32;   // tile columns
+constexpr int OZ_BN_SINGLE = 64;
 constexpr int OZ_ASLOTS = 4;   // A ring depth
 constexpr int OZ_A_TILE = OZ_BM * OZ_BK;  // 16 KB
-// tile columns per accumulator: 64 with 8 slices (double), 128 with 4 (single)
 
 // ------------------------------------------------------------------ PTX ----
 __device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
@@ -91,46 +93,69 @@ __device__ __forceinline__ void tma_load_3d(void *dst, const CUtensorMap *map,
       "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                        uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+}
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+
+// D(64 x BN, s32, registers) += A(64 x 32, s8, smem) * B(32 x BN, s8, smem),
+// both operands K-major.  Thread t of the warpgroup holds, for every 8-column
+// chunk j, d[4j + 2h + e] = D[16 (t/32) + (t%32)/4 + 8h][8j + 2 (t%4) + e].
+template <int BN>
+__device__ __forceinline__ void wgmma_s8(int32_t (&d)[BN / 2], uint64_t adesc, uint64_t bdesc);
+
+template <>
+__device__ __forceinline__ void wgmma_s8<32>(int32_t (&d)[16], uint64_t adesc, uint64_t bdesc) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p;\n"
+      "}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]),
+        "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]),
+        "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(1)
       : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, int32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]),
-        "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_100 format):
-// start>>4 [0,14), LBO [16,30) = 1 (unused), SBO [32,46) = 1024>>4 (8 rows of
-// 128 B), version [46,48) = 1, layout type [61,64) = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) |
-         (1ull << 46) | (2ull << 61);
+template <>
+__device__ __forceinline__ void wgmma_s8<64>(int32_t (&d)[32], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p;\n"
+      "}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]),
+        "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]),
+        "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]),
+        "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]),
+        "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]),
+        "+r"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(1)
+      : "memory");
+}
+
+// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_90 wgmma format):
+// start>>4 [0,14), LBO [16,30) = 1 (unused for swizzled K-major), SBO [32,46)
+// = 1024>>4 (8 rows of 128 B), base offset [49,52) = 0 (1024-aligned tiles),
+// layout type [62,64) = 1 (SWIZZLE_128B).  A K step of 32 bytes inside the
+// 128-byte swizzle row advances the start address by 2.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
 
 // --------------------------------------------------- operand preparation ----
@@ -306,88 +331,87 @@ struct OzGemmParams {
   const double *scaleB;   // [Npad]
 };
 
-template <int BN>
+// BN output columns per CTA, NSL accumulators (the most slices the
+// instantiation takes): NSL x BN/2 = 128 accumulator registers per consumer
+// thread -- 32 columns with 8 slices (double), 64 with 4 (single).
+template <int BN, int NSL>
 struct OzSmem {
-  static constexpr int B_TILE = BN * OZ_BK;               // 8 / 16 KB
-  static constexpr int NS = 512 / BN;                     // slices that fit TMEM
-  static constexpr size_t TILES = (size_t)OZ_ASLOTS * OZ_A_TILE + 2 * (size_t)NS * B_TILE;
+  static constexpr int B_TILE = BN * OZ_BK;               // 4 / 8 KB
+  static constexpr size_t TILES = (size_t)OZ_ASLOTS * OZ_A_TILE + 2 * (size_t)NSL * B_TILE;
   static constexpr size_t BYTES = TILES + 1024 /*align*/ + 8192 /*tables, barriers*/;
 };
 
-template <int BN, typename OutT>
-__global__ void __launch_bounds__(192, 1)
+constexpr int OZ_THREADS = 384;    // producer warpgroup + 2 consumer warpgroups
+constexpr int OZ_CONSUMER_WARPS = 8;
+
+template <int BN, int NSL, typename OutT>
+__global__ void __launch_bounds__(OZ_THREADS, 1)
     ozaki_gemm_kernel(const __grid_constant__ CUtensorMap mapA,
                       const __grid_constant__ CUtensorMap mapB,
                       const __grid_constant__ OzGemmParams P) {
-  constexpr int B_TILE = OzSmem<BN>::B_TILE;
-  constexpr int NS = OzSmem<BN>::NS;
+  constexpr int B_TILE = OzSmem<BN, NSL>::B_TILE;
   extern __shared__ unsigned char oz_smem_raw[];
   unsigned char *base = reinterpret_cast<unsigned char *>(
       ((uintptr_t)oz_smem_raw + 1023) & ~(uintptr_t)1023);
   unsigned char *sA = base;                                   // 4 x 16 KB
-  unsigned char *sB = base + (size_t)OZ_ASLOTS * OZ_A_TILE;   // 2 x NS x B_TILE
-  unsigned char *aux = base + OzSmem<BN>::TILES;
+  unsigned char *sB = base + (size_t)OZ_ASLOTS * OZ_A_TILE;   // 2 x NSL x B_TILE
+  unsigned char *aux = base + OzSmem<BN, NSL>::TILES;
   uint64_t *fullA = reinterpret_cast<uint64_t *>(aux);        // [4]
   uint64_t *emptyA = fullA + OZ_ASLOTS;                       // [4]
   uint64_t *fullB = emptyA + OZ_ASLOTS;                       // [2]
   uint64_t *emptyB = fullB + 2;                               // [2]
-  uint64_t *tmem_full = emptyB + 2;                           // [1]
-  uint32_t *tmem_base_s = reinterpret_cast<uint32_t *>(tmem_full + 1);
   int64_t *offCm = reinterpret_cast<int64_t *>(aux + 256);    // [128]
   int64_t *offCn = offCm + OZ_BM;                             // [BN]
   double *sclM = reinterpret_cast<double *>(offCn + BN);      // [128]
   double *sclN = sclM + OZ_BM;                                // [BN]
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
   const int S = P.S, nkb = P.nkb;
   const int tm = blockIdx.x, tn = blockIdx.y;
 
   if (tid == 0) {
-    for (int i = 0; i < OZ_ASLOTS; ++i) { mbar_init(&fullA[i], 1); mbar_init(&emptyA[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], 1); }
-    mbar_init(tmem_full, 1);
+    for (int i = 0; i < OZ_ASLOTS; ++i) {
+      mbar_init(&fullA[i], 1);
+      mbar_init(&emptyA[i], OZ_CONSUMER_WARPS);
+    }
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&fullB[i], 1);
+      mbar_init(&emptyB[i], OZ_CONSUMER_WARPS);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tmem_base_s)),
-                 "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  // epilogue tables (warps 2..5 = 128 threads); offsets in units of OutT
-  if (warp >= 2) {
-    const int e = tid - 64;
+  // epilogue tables (consumer threads); offsets in units of OutT
+  if (tid >= 128) {
+    const int e = tid - 128;
     const int csh = P.cplx ? 1 : 0;
-    {
+    if (e < OZ_BM) {
       const int64_t m = (int64_t)tm * OZ_BM + e;
       int64_t oa, oc = -1;
       if (m < P.Me) { decode2(m, P.c.m, oa, oc); oc <<= csh; }
       offCm[e] = oc;
       sclM[e] = P.scaleA[(int64_t)tm * OZ_BM + e];
-    }
-    if (e < BN) {
-      const int64_t ne = (int64_t)tn * BN + e;
+    } else if (e - OZ_BM < BN) {
+      const int c = e - OZ_BM;
+      const int64_t ne = (int64_t)tn * BN + c;
       int64_t ob, oc = -1;
       if (ne < P.Ne) { decode2(ne >> csh, P.c.n, ob, oc); oc = (oc << csh) + (csh ? (ne & 1) : 0); }
-      offCn[e] = oc;
-      sclN[e] = P.scaleB[(int64_t)tn * BN + e];
+      offCn[c] = oc;
+      sclN[c] = P.scaleB[(int64_t)tn * BN + c];
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_s;
 
-  if (warp == 0) {
-    // =========================== TMA producer ==============================
-    if (lane == 0) {
+  if (tid < 128) {
+    // ======================= TMA producer warpgroup ========================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (tid == 0) {
       int ia = 0;
       for (int kb = 0; kb < nkb; ++kb) {
         const int sb = kb & 1;
         mbar_wait(&emptyB[sb], ((kb >> 1) & 1) ^ 1);
         mbar_expect_tx(&fullB[sb], (uint32_t)S * B_TILE);
         for (int q = 0; q < S; ++q)
-          tma_load_3d(sB + ((size_t)sb * NS + q) * B_TILE, &mapB, &fullB[sb],
+          tma_load_3d(sB + ((size_t)sb * NSL + q) * B_TILE, &mapB, &fullB[sb],
                       kb * OZ_BK, tn * BN, q);
         for (int p = 0; p < S; ++p, ++ia) {
           const int sa = ia % OZ_ASLOTS;
@@ -398,82 +422,91 @@ __global__ void __launch_bounds__(192, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ============================ MMA issuer ================================
-    if (lane == 0) {
-      // kind::i8: D = S32 (2<<4), A = INT8 (1<<7), B = INT8 (1<<10), K-major
-      // both, N>>3 at [17,23), M>>4 at [24,29)
-      const uint32_t idesc = (2u << 4) | (1u << 7) | (1u << 10) |
-                             ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(OZ_BM >> 4) << 24);
-      int ia = 0;
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int sb = kb & 1;
-        mbar_wait(&fullB[sb], (kb >> 1) & 1);
-        tc_fence_after();
-        for (int p = 0; p < S; ++p, ++ia) {
-          const int sa = ia % OZ_ASLOTS;
-          mbar_wait(&fullA[sa], (ia / OZ_ASLOTS) & 1);
-          tc_fence_after();
-          const uint64_t adesc = umma_desc_sw128(smem_u32(sA + (size_t)sa * OZ_A_TILE));
-          for (int q = 0; q + p < S; ++q) {
-            const uint64_t bdesc =
-                umma_desc_sw128(smem_u32(sB + ((size_t)sb * NS + q) * B_TILE));
-            const uint32_t dcol = tmem_base + (uint32_t)(p + q) * BN;
-#pragma unroll
-            for (int k4 = 0; k4 < OZ_BK / 32; ++k4) {
-              // first touch of accumulator d = p+q is (kb=0, p=0, k4=0)
-              const uint32_t accum = (kb > 0 || p > 0 || k4 > 0) ? 1u : 0u;
-              umma_i8(dcol, adesc + (uint64_t)(k4 * 2), bdesc + (uint64_t)(k4 * 2), idesc,
-                      accum);
-            }
-          }
-          umma_commit(&emptyA[sa]);  // slot free once these MMAs retire
-        }
-        umma_commit(&emptyB[sb]);
-      }
-      umma_commit(tmem_full);
-    }
-  } else {
-    // ============================== epilogue ================================
-    const int quarter = warp & 3;          // TMEM lane quarter this warp may access
-    const int row = quarter * 32 + lane;   // row of the tile = TMEM lane
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    const int64_t om = offCm[row];
-    const double sm = sclM[row] * P.c.alpha;
-    OutT *C = static_cast<OutT *>(P.c.C);
-    const double beta = P.c.beta;
-    for (int cc = 0; cc < BN; cc += 16) {
-      double acc[16];
-#pragma unroll
-      for (int i = 0; i < 16; ++i) acc[i] = 0.0;
-      double w = ldexp(1.0, -7 * (S - 1));
-      for (int d = S - 1; d >= 0; --d) {
-        int32_t v[16];
-        tmem_ld16(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(d * BN + cc), v);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[i] += w * (double)v[i];
-        w *= 128.0;
-      }
-      if (om >= 0) {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int64_t on = offCn[cc + i];
-          if (on >= 0) {
-            double val = acc[i] * sm * sclN[cc + i];
-            if (beta != 0.0) val += beta * (double)C[om + on];
-            C[om + on] = (OutT)val;
-          }
-        }
-      }
-    }
-    tc_fence_before();
+    return;
   }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(512));
+  // ===================== consumer warpgroups (wgmma) ======================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int ct = tid - 128;
+  const int half = ct >> 7;          // rows [64 half, 64 half + 64) of the tile
+  const int wq = (ct >> 5) & 3;      // warp within the warpgroup
+  int32_t acc[NSL][BN / 2];
+#pragma unroll
+  for (int d = 0; d < NSL; ++d)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[d][i] = 0;
+
+  // for p: for q <= S-1-p: acc[p+q] += A_p B_q, one commit group per A slice;
+  // a slot is released once the group after it has been issued and the
+  // group using it has retired (wgmma.wait_group 1)
+  int ia = 0, pend_a = -1, pend_b = -1;
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int sb = kb & 1;
+    mbar_wait(&fullB[sb], (kb >> 1) & 1);
+#pragma unroll
+    for (int p = 0; p < NSL; ++p) {
+      if (p < S) {
+        const int sa = ia % OZ_ASLOTS;
+        mbar_wait(&fullA[sa], (ia / OZ_ASLOTS) & 1);
+        const uint64_t adesc = wgmma_desc_sw128(
+            smem_u32(sA + (size_t)sa * OZ_A_TILE + (size_t)half * 64 * OZ_BK));
+        wgmma_fence();
+#pragma unroll
+        for (int q = 0; q < NSL; ++q) {
+          if (p + q < S) {
+            const uint64_t bdesc =
+                wgmma_desc_sw128(smem_u32(sB + ((size_t)sb * NSL + q) * B_TILE));
+#pragma unroll
+            for (int k4 = 0; k4 < OZ_BK / 32; ++k4)
+              wgmma_s8<BN>(acc[p + q], adesc + (uint64_t)(k4 * 2), bdesc + (uint64_t)(k4 * 2));
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (lane == 0) {
+          if (pend_a >= 0) mbar_arrive(&emptyA[pend_a]);
+          if (pend_b >= 0) mbar_arrive(&emptyB[pend_b]);
+        }
+        pend_a = sa;
+        pend_b = (p == S - 1) ? sb : -1;
+        ++ia;
+      }
+    }
+  }
+  wgmma_wait<0>();
+
+  // ============================== epilogue ================================
+  // combine the S accumulators in fp64 with exact power-of-two weights,
+  // apply the row / column scales and alpha/beta, scatter to the strided C
+  OutT *C = static_cast<OutT *>(P.c.C);
+  const double beta = P.c.beta;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = half * 64 + wq * 16 + (lane >> 2) + 8 * h;
+    const int64_t om = offCm[row];
+    if (om < 0) continue;
+    const double sm = sclM[row] * P.c.alpha;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int i = 4 * j + 2 * h + e;
+        const int col = 8 * j + 2 * (lane & 3) + e;
+        double v = 0.0, w = ldexp(1.0, -7 * (S - 1));
+#pragma unroll
+        for (int d = NSL - 1; d >= 0; --d) {
+          if (d < S) {
+            v += w * (double)acc[d][i];
+            w *= 128.0;
+          }
+        }
+        const int64_t on = offCn[col];
+        if (on >= 0) {
+          double val = v * sm * sclN[col];
+          if (beta != 0.0) val += beta * (double)C[om + on];
+          C[om + on] = (OutT)val;
+        }
+      }
+    }
   }
 }
 
@@ -534,7 +567,7 @@ static int oz_slices(bool single) {
   static int s4 = [] {
     const char *e = getenv("QB_OZAKI_SLICES_SINGLE");
     int v = e ? atoi(e) : 4;
-    return std::max(2, std::min(v, 4));
+    return std::max(2, std::min(v, OZ_MAXS_SINGLE));
   }();
   return single ? s4 : s8;
 }
@@ -545,7 +578,7 @@ static void oz_geometry(const PairPlan &plan, OzGeom &g) {
   g.single = (plan.dtype == QB_F32 || plan.dtype == QB_C64) ? 1 : 0;
   g.cplx = dtype_is_complex(plan.dtype) ? 1 : 0;
   g.S = oz_slices(g.single);
-  g.BN = g.single ? 128 : 64;
+  g.BN = g.single ? OZ_BN_SINGLE : OZ_BN_DOUBLE;
   g.Me = p.M;
   g.Ne = g.cplx ? 2 * p.N : p.N;
   g.Ke = g.cplx ? 2 * p.K : p.K;
@@ -575,17 +608,17 @@ int64_t ozaki_workspace_bytes(const PairPlan &plan) {
   return g.total;
 }
 
-template <int BN, typename OutT>
+template <int BN, int NSL, typename OutT>
 static int oz_launch_gemm(const CUtensorMap &mapA, const CUtensorMap &mapB,
                           const OzGemmParams &gp, dim3 grid, cudaStream_t st) {
-  auto kern = ozaki_gemm_kernel<BN, OutT>;
+  auto kern = ozaki_gemm_kernel<BN, NSL, OutT>;
   static bool attr_set = false;
   if (!attr_set) {
     QB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)OzSmem<BN>::BYTES));
+                                       (int)OzSmem<BN, NSL>::BYTES));
     attr_set = true;
   }
-  kern<<<grid, 192, OzSmem<BN>::BYTES, st>>>(mapA, mapB, gp);
+  kern<<<grid, OZ_THREADS, OzSmem<BN, NSL>::BYTES, st>>>(mapA, mapB, gp);
   QB_LAUNCH_CHECK();
   return 0;
 }
@@ -658,8 +691,8 @@ int launch_contract_ozaki(const PairPlan &plan, void *workspace, cudaStream_t st
   gp.scaleA = reinterpret_cast<const double *>(ws + g.off_scA);
   gp.scaleB = reinterpret_cast<const double *>(ws + g.off_scB);
   dim3 grid((unsigned)(g.Mpad / OZ_BM), (unsigned)((g.Ne + g.BN - 1) / g.BN));
-  if (g.single) return oz_launch_gemm<128, float>(mapA, mapB, gp, grid, st);
-  return oz_launch_gemm<64, double>(mapA, mapB, gp, grid, st);
+  if (g.single) return oz_launch_gemm<OZ_BN_SINGLE, OZ_MAXS_SINGLE, float>(mapA, mapB, gp, grid, st);
+  return oz_launch_gemm<OZ_BN_DOUBLE, OZ_MAXS, double>(mapA, mapB, gp, grid, st);
 }
 
 }  // namespace qb

@@ -116,6 +116,10 @@ static const TileCfg kTileCfgs[] = {
 };
 constexpr int kNumTileCfgs = 5;
 
+// fp64 tensor-core rate of one SM per microsecond: H100 SXM, 128 DMMA FMA per
+// clock at the 1.98 GHz boost clock (data sheet: 67 TFLOP/s over 132 SMs)
+constexpr double kDmmaFmaPerSmUs = 128.0 * 1980.0;
+
 // k-depth of the large tile: 32 (3 stages) or 16 (4 stages); QB_CFG0_BK
 // overrides for tuning
 inline int cfg0_bk() {
@@ -325,11 +329,12 @@ inline int plan_pair(const qb_tensor_t *A, const int32_t *la,
   const int64_t M = p.M, N = cplx ? 2 * p.N : p.N, Kh = cplx ? 2 * p.K : p.K;
   // cost model: time ~ waves * (padded tile work) / (per-CTA rate), plus the
   // split-K partial write + reduce traffic.  occ = resident CTAs per SM,
-  // eff = measured fraction of the DMMA peak at full occupancy (B200).
+  // eff = assumed fraction of the DMMA peak at full occupancy.
   static const int kOcc[kNumTileCfgs] = {1, 2, 2, 2, 5};
   static const double kEff[kNumTileCfgs] = {0.73, 0.60, 0.50, 0.50, 0.30};
-  const double kFmaPerUs = 148.0 * 64.0 * 1965.0;  // chip FMA rate / us
-  const double kBytesPerUs = 5.0e6;                // ~5 TB/s for the reduce
+  const int nsm = sm_count();
+  const double kFmaPerUs = nsm * kDmmaFmaPerSmUs;  // chip FMA rate / us
+  const double kBytesPerUs = 3.35e6;  // HBM3 bandwidth of the H100 SXM data sheet
   double best_t = 1e300;
   int best_cfg = 1, best_split = 1;
   int64_t best_kper = 0;
@@ -338,7 +343,7 @@ inline int plan_pair(const qb_tensor_t *A, const int32_t *la,
     const TileCfg tc = tile_cfg(c);
     const int64_t tiles = cdiv(M, tc.bm) * cdiv(N, tc.bn) * p.nbatch;
     const int64_t kblocks = std::max<int64_t>(cdiv(Kh, tc.bk), 1);
-    const int64_t slots = 148LL * kOcc[c];
+    const int64_t slots = (int64_t)nsm * kOcc[c];
     for (int64_t sk = 1; sk <= max_splitk; sk *= 2) {
       if (sk > 1 && (kblocks / sk < 4)) break;
       const int64_t kb_per = cdiv(kblocks, sk);
@@ -347,10 +352,10 @@ inline int plan_pair(const qb_tensor_t *A, const int32_t *la,
       const double waves = (double)cdiv(units, slots);
       // CTAs only share an SM when there are enough of them; a lone CTA
       // is capped by how many of the 4 sub-partitions its warps cover
-      const double share = (double)std::min<int64_t>(kOcc[c], cdiv(units, 148));
+      const double share = (double)std::min<int64_t>(kOcc[c], cdiv(units, nsm));
       const double warpcap = std::min(1.0, (tc.threads / 32) / 4.0) * 0.8;
       const double cta_rate =
-          kFmaPerUs / 148.0 * std::min(kEff[c] / share, warpcap);
+          kDmmaFmaPerSmUs * std::min(kEff[c] / share, warpcap);
       double t = waves * ((double)tc.bm * tc.bn * kb_per * tc.bk) / cta_rate;
       t += 3.0;  // launch latency
       if (nsplit > 1)
@@ -377,7 +382,9 @@ inline int plan_pair(const qb_tensor_t *A, const int32_t *la,
       const char *e = getenv("QB_STREAMK");
       return e ? atoi(e) : 1;
     }();
-    const int G = 148;
+    // one persistent CTA per SM: owners spin on their peers' flags, so every
+    // CTA of the grid must be resident at once
+    const int G = nsm;
     const int64_t tiles = (int64_t)p.tiles_m * p.tiles_n;
     const int64_t kblocks = cdiv(Kh, tc.bk);
     const double eff = (double)(tiles * p.splitk) / (double)(cdiv(tiles * p.splitk, G) * G);
@@ -387,13 +394,14 @@ inline int plan_pair(const qb_tensor_t *A, const int32_t *la,
       p.splitk = 1;
       p.k_per_split = kblocks * tc.bk;
       // fix-up (wait + collect the peers' partial tiles) + epilogue of a
-      // shared tile cost its owner ~9 us = this many k-blocks (measured with
-      // the in-kernel trace); it gets that much less of the main loop
+      // shared tile cost its owner about head_us = this many k-blocks; it gets
+      // that much less of the main loop.  9 us is an estimate that has not
+      // been measured on the H100 (QB_SK_HEAD_US overrides it for tuning)
       static const int head_us = [] {
         const char *e = getenv("QB_SK_HEAD_US");
         return e ? atoi(e) : 9;
       }();
-      const double kb_us = (double)tc.bm * tc.bn * tc.bk / (64.0 * 0.9) / 1965.0;
+      const double kb_us = (double)tc.bm * tc.bn * tc.bk / (0.9 * kDmmaFmaPerSmUs);
       int64_t H = (int64_t)(head_us / kb_us + 0.5);
       const int64_t share = tiles * (kblocks + H) / G;
       if (H >= share / 2) H = 0;

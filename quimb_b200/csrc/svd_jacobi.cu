@@ -16,7 +16,7 @@
 //     overlaps the DMMA-bound Gram / apply phases of others -- the phases of
 //     one launch all coincide, which is what left the tensor pipe 33 % busy;
 //   * a column-block pair is owned by a CLUSTER of 4 or 8 CTAs (rows dealt in
-//     chunks), 256 or 512 CTAs per round over all streams: all 148 SMs busy;
+//     chunks), 256 or 512 CTAs per round over all streams: every SM busy;
 //   * the partial Gram is computed with each warp owning one 16 x 8 output
 //     tile over all rows of the chunk: no cross-warp reduction, only the
 //     fixed-order cluster reduction through distributed shared memory;

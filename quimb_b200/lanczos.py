@@ -25,7 +25,7 @@ process lives on the device here:
 
 Convergence test as in ARPACK's dsaupd: ``resid <= tol * max(eps^(2/3),
 |theta|)``.  The basis size ``ncv`` is a free parameter of the device solver:
-ARPACK's 4 is memory-frugal for host vectors; on a 180 GB device a basis of
+ARPACK's 4 is memory-frugal for host vectors; on an 80 GB device a basis of
 8-16 vectors (32 MiB each at chi = 1024) needs far fewer matvecs.
 ``eigh_arpack_host_driver`` is the parity mode (scipy ARPACK on the host
 driving the device matvec).

@@ -289,7 +289,7 @@ class MovingEnvironment:
     ``envs`` maps a window start ``i`` to ``(L_i, R_i)`` with L_i the
     contraction of sites < i and R_i of sites >= i + bsz.  Like the reference,
     environments of visited positions stay cached (40 MiB each at chi = 1024,
-    w = 5: 4 GB for L = 100 out of 180 GB) and are overwritten when the window
+    w = 5: 4 GB for L = 100 out of an 80 GB device) and are overwritten when the window
     comes back after the sites changed."""
 
     def __init__(self, sites, mpo, begin="left", bsz=2):

@@ -382,7 +382,8 @@ def _optimal_ssa(inputs, output, size_dict):
 # multiply-add equivalents charged per intermediate element by the 'combo'
 # objective of the device-targeted searches: a complex128 element written and
 # read back costs 2 x 16 B / (HBM bytes/s) against 8 flop / (fp64 flop/s) per
-# multiply-add, about 14 on a B200 (7.7 TB/s, 25-33 TFLOP/s measured)
+# multiply-add; 16 is that ratio rounded for an HBM-bandwidth to fp64-rate
+# ratio like the H100 data sheet's (3.35 TB/s, 67 TFLOP/s)
 DEVICE_COMBO = ("combo", 16.0)
 
 

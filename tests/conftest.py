@@ -13,7 +13,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (B200)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (H100)")
 
 
 def pytest_collection_modifyitems(config, items):

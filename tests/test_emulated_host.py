@@ -19,7 +19,7 @@ from tests.abi_emulator import emulated_abi
 _SKIP = {
     "test_gpu_contract": {
         "test_full_size_properties_chi1024",
-        # assert the launch count of the tcgen05 engine's kernel sequence
+        # assert the launch count of the int8 engine's kernel sequence
         "test_tcgen05_engine_matches_oracle",
         "test_tcgen05_engine_badly_scaled_and_accumulate",
         "test_native_single_precision_engine",

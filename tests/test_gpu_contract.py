@@ -229,7 +229,7 @@ def test_full_size_properties_chi1024():
     assert float(abs(a - b).max().item()) < 1e-10
 
 
-# ---- tcgen05 (int8 error-free split) engine -------------------------------
+# ---- int8 (error-free split) engine -------------------------------------
 OZ_CASES = [
     ("ab,bc->ac", dict(a=128, b=128, c=64)),
     ("ab,bc->ac", dict(a=1000, b=777, c=333)),
@@ -251,7 +251,7 @@ def test_tcgen05_engine_matches_oracle(eq, sizes):
     n0 = qb.launch_count()
     out = qb.contract_pair(A.t, [sym[c] for c in ta], B.t, [sym[c] for c in tb],
                            [sym[c] for c in rhs], engine=2)
-    # rowmax + split for each operand, then the tcgen05 GEMM: 5 launches
+    # rowmax + split for each operand, then the int8 GEMM: 5 launches
     assert qb.launch_count() - n0 == 5
     ref = np.einsum(eq, a, b)
     # fp64-level: error relative to max|row| max|col| sqrt(K)
@@ -322,7 +322,7 @@ def test_single_precision_dtype_preserved(dtype, tol):
     assert np.max(np.abs(out2.to_numpy() - ref2)) <= 10 * tol * np.max(np.abs(ref2))
 
 
-# ---- native single precision / complex on the tcgen05 engine ---------------
+# ---- native single precision / complex on the int8 engine ------------------
 SINGLE_CASES = [
     ("ab,bc->ac", dict(a=256, b=192, c=160)),
     ("ba,bc->ca", dict(a=300, b=200, c=150)),
@@ -335,7 +335,7 @@ SINGLE_CASES = [
 @pytest.mark.parametrize("eq,sizes", SINGLE_CASES)
 def test_native_single_precision_engine(eq, sizes, dtype):
     """float32 / complex64 contractions above the tile minimum run on the
-    tcgen05 engine directly (4 int8 slices, float epilogue): 5 launches, no
+    int8 engine directly (4 int8 slices, float epilogue): 5 launches, no
     conversion passes; result at fp32 accuracy of the exact product (the
     reference's numpy path rounds every partial sum to fp32, this rounds once)."""
     rng = np.random.default_rng(abs(hash(eq + dtype)) % 2**31)

@@ -20,6 +20,7 @@ import pytest
 import torch
 
 import quimb_b200 as qb
+from quimb_b200 import _lib
 from oracle import decomp_np as dn
 from oracle import dmrg_np as dm
 
@@ -155,21 +156,31 @@ def test_dmrg2_two_site_update_at_chi1024_vs_numpy():
     assert _rel(E, Eref) < 1e-11
 
 
-def test_cfg1_4096_cubed_takes_the_tcgen05_engine_by_default():
+def test_cfg1_4096_cubed_default_dmma_and_int8_engine():
     """BASELINE configs[0] at full size: two rank-4 chi=64 tensors sharing two
-    indices = a 4096^3 GEMM.  Above 1e11 flops `engine=auto` is the tcgen05
-    int8-split engine (5 launches: row maxima + split of each operand, GEMM);
-    result at fp64 level against numpy."""
+    indices = a 4096^3 GEMM.  `engine=auto` runs float64 on the DMMA kernel
+    (one launch, plus a reduce when split-K is chosen); the int8-split engine,
+    requested explicitly, takes 5 launches (row maxima + split of each
+    operand, GEMM).  Both at fp64 level against numpy."""
     rng = np.random.default_rng(15)
     a = rng.standard_normal((64, 64, 64, 64))
     b = rng.standard_normal((64, 64, 64, 64))
     A, B = qb.asarray(a), qb.asarray(b)
+    ref = np.tensordot(a, b, axes=((2, 3), (0, 1)))
     n0 = qb.launch_count()
     out = qb.tensordot(A, B, axes=((2, 3), (0, 1)))
-    assert qb.launch_count() - n0 == 5
-    ref = np.tensordot(a, b, axes=((2, 3), (0, 1)))
+    assert qb.launch_count() - n0 <= 2
     assert _rel(out.to_numpy(), ref) < 1e-12
+    n0 = qb.launch_count()
+    out8 = qb.contract_pair(A.t, [0, 1, 2, 3], B.t, [2, 3, 4, 5], [0, 1, 4, 5],
+                            engine=_lib.QB_ENGINE_OZAKI)
+    assert qb.launch_count() - n0 == 5
+    assert _rel(out8.cpu().numpy(), ref) < 1e-12
     # permuted operands (the index permutation is folded into the split gather)
-    out2 = qb.tensordot(A.transpose(0, 2, 1, 3), B.transpose(3, 1, 2, 0), axes=((1, 3), (3, 2)))
     ref2 = np.tensordot(a.transpose(0, 2, 1, 3), b.transpose(3, 1, 2, 0), axes=((1, 3), (3, 2)))
+    out2 = qb.tensordot(A.transpose(0, 2, 1, 3), B.transpose(3, 1, 2, 0), axes=((1, 3), (3, 2)))
     assert _rel(out2.to_numpy(), ref2) < 1e-12
+    out28 = qb.contract_pair(A.t.permute(0, 2, 1, 3), [0, 1, 2, 3],
+                             B.t.permute(3, 1, 2, 0), [4, 5, 3, 1], [0, 2, 4, 5],
+                             engine=_lib.QB_ENGINE_OZAKI)
+    assert _rel(out28.cpu().numpy(), ref2) < 1e-12

@@ -1,8 +1,8 @@
 """PEPS boundary-MPS contraction benchmark (BASELINE configs[4]: 10x10 PEPS,
-bond 8, boundary chi 256, complex64).  Not the driver's bench.py contract
-(that is configs[1]); run under gpurun:
+bond 8, boundary chi 128, complex64 -- sized for one 80 GB GPU; at chi 256 the
+intermediates need more than 80 GB).  bench.py measures configs[1]:
 
-  python tools/bench_boundary.py [--Lx 10] [--Ly 10] [--D 8] [--chi 256]
+  python tools/bench_boundary.py [--Lx 10] [--Ly 10] [--D 8] [--chi 128]
                                  [--dtype complex64] [--reps 1]
   torchrun --nproc-per-node 2 tools/bench_boundary.py --two-sided
 
@@ -53,7 +53,7 @@ def main():
     ap.add_argument("--Lx", type=int, default=10)
     ap.add_argument("--Ly", type=int, default=10)
     ap.add_argument("--D", type=int, default=8)
-    ap.add_argument("--chi", type=int, default=256)
+    ap.add_argument("--chi", type=int, default=128)
     ap.add_argument("--dtype", default="complex64")
     ap.add_argument("--reps", type=int, default=1)
     ap.add_argument("--two-sided", action="store_true")

@@ -36,7 +36,7 @@ def main():
     ap.add_argument("--target-width", type=int, default=28)
     ap.add_argument("--max-slices", type=int, default=64)
     ap.add_argument("--reps", type=int, default=1)
-    ap.add_argument("--max-gb", type=float, default=140.0,
+    ap.add_argument("--max-gb", type=float, default=70.0,
                     help="refuse trees whose live intermediates exceed this many GB")
     ap.add_argument("--out", default=None)
     ap.add_argument("--tree-file", default=None,
