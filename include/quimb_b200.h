@@ -158,6 +158,26 @@ int qb_contract_pair_plan(const qb_tensor_t *A, const int32_t *labelsA,
                           int64_t *out16);
 
 /*
+ * Host-only: the kernel route qb_contract_pair takes for these operands and
+ * this engine argument (given a large enough workspace).  The launch path
+ * and this report come from the same decision function.
+ * out[0] = route kind: 0 empty output, 1 zero fill, 2 widen (single
+ *          precision below the int8 engine's minimum: the caller widens),
+ *          3 int8 engine, 4 streaming engine, 5 DMMA classic grid,
+ *          6 DMMA stream-K grid
+ * out[1] = DMMA tile config (-1 otherwise), out[2] = split-K factor,
+ * out[3] = stream-K grid (CTAs, 0 otherwise), out[4] = stream-K head cost
+ * (k-blocks), out[5] = DMMA k-block depth, out[6] = cfg-0 shared-memory
+ * layout of real operands (a_kmajor * 2 + b_kmajor; -1: runtime layout),
+ * out[7] = SM count the planner used, out[8] = kernels launched (beta = 0).
+ * The caller provides 16 slots.
+ */
+int qb_contract_pair_route(const qb_tensor_t *A, const int32_t *labelsA,
+                           const qb_tensor_t *B, const int32_t *labelsB,
+                           const qb_tensor_t *C, const int32_t *labelsC,
+                           int engine, int64_t *out16);
+
+/*
  * TEST / debug entry, host pointers only: runs the streaming engine's row
  * code (shared __host__ __device__ functions of contract_stream.cu) in a
  * host loop so that its index bookkeeping can be checked without a device.

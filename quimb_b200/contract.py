@@ -274,6 +274,33 @@ def plan_pair(a_shape, a_strides, la, b_shape, b_strides, lb, c_shape,
     return dict(zip(keys, list(out)))
 
 
+ROUTE_KINDS = ("empty", "zero_fill", "widen", "int8", "stream", "dmma", "dmma_streamk")
+
+
+def route_pair(a_shape, a_strides, la, b_shape, b_strides, lb, c_shape,
+               c_strides, lc, dtype_code=_lib.QB_F64, engine=0, ptrs=None):
+    """Host-only: the kernel route ``contract_pair`` takes for operands of
+    these shapes and strides (the library's own dispatch decision, at the SM
+    count of the current device or the H100 SXM's 132 without one).
+
+    ``ptrs`` = (a, b, c) base addresses; the vector loads depend on 16-byte
+    alignment, so pass the real ones when the route of a view matters."""
+    lib = _lib.load()
+    pa, pb, pc = ptrs if ptrs is not None else (0x10000000,) * 3
+    da = _lib.np_desc(a_shape, a_strides, dtype_code, pa)
+    db = _lib.np_desc(b_shape, b_strides, dtype_code, pb)
+    dc = _lib.np_desc(c_shape, c_strides, dtype_code, pc)
+    out = (ctypes.c_int64 * 16)()
+    rc = lib.qb_contract_pair_route(da, _lib.labels(la), db, _lib.labels(lb),
+                                    dc, _lib.labels(lc), int(engine), out)
+    _lib.check(rc, "qb_contract_pair_route")
+    keys = ("kind", "cfg", "splitk", "streamk", "sk_head", "bk", "layout", "sms",
+            "launches")
+    r = dict(zip(keys, list(out)))
+    r["kind"] = ROUTE_KINDS[r["kind"]]
+    return r
+
+
 def contract_batched(a_list, la, b_list, lb, lc, conj_a=False, conj_b=False):
     """Many independent contractions of identical signature in ONE launch
     (the small same-shape intermediates of MPS / PEPS / circuit sweeps).

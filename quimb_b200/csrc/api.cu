@@ -117,6 +117,36 @@ static bool want_stream(int engine, const PairPlan &plan) {
   return engine == QB_ENGINE_STREAM && stream_eligible(plan);
 }
 
+// QB_FORCE_CFG: tuning/debug override of the tile configuration
+static int force_cfg() {
+  static const int v = [] {
+    const char *e = getenv("QB_FORCE_CFG");
+    return e ? atoi(e) : -1;
+  }();
+  return v;
+}
+
+// The one dispatch decision of a pairwise contraction (engine = the low byte
+// of the caller's engine argument).  contract_pair_impl launches what this
+// returns and qb_contract_pair_route reports it.
+static Route select_route(const PairPlan &plan, int engine) {
+  Route r{ROUTE_DMMA, -1, 1, 0, 0, 0, -1, 0};
+  if (plan.empty_out) { r.kind = ROUTE_EMPTY; return r; }
+  if (plan.zero_fill) {
+    r.kind = ROUTE_ZERO_FILL;
+    r.launches = plan.out_elems > 0 ? 1 : 0;
+    return r;
+  }
+  if (is_single(plan.dtype) && !ozaki_eligible(plan)) { r.kind = ROUTE_WIDEN; return r; }
+  if (want_ozaki(engine, plan)) {
+    r.kind = ROUTE_INT8;
+    r.launches = 5;  // rowmax + split of each operand, then the int8 GEMM
+    return r;
+  }
+  if (want_stream(engine, plan)) { r.kind = ROUTE_STREAM; r.launches = 1; return r; }
+  return dmma_route(plan, true);
+}
+
 
 extern "C" {
 
@@ -137,6 +167,20 @@ int qb_contract_pair_plan(const qb_tensor_t *A, const int32_t *la,
   out[8] = plan.cfg; out[9] = p.splitk; out[10] = p.vecA; out[11] = p.vecB;
   out[12] = p.vecC; out[13] = p.thrA; out[14] = p.thrB;
   out[15] = plan.empty_out ? 2 : (plan.zero_fill ? 1 : 0);
+  return 0;
+}
+
+int qb_contract_pair_route(const qb_tensor_t *A, const int32_t *la,
+                           const qb_tensor_t *B, const int32_t *lb,
+                           const qb_tensor_t *C, const int32_t *lc, int engine,
+                           int64_t *out) {
+  PairPlan plan;
+  int rc = plan_pair(A, la, B, lb, C, lc, 0, 0, plan, force_cfg());
+  if (rc) return rc;
+  const Route r = select_route(plan, engine & 0xff);
+  out[0] = r.kind; out[1] = r.cfg; out[2] = r.splitk; out[3] = r.streamk;
+  out[4] = r.sk_head; out[5] = r.bk; out[6] = r.layout; out[7] = sm_count();
+  out[8] = r.launches;
   return 0;
 }
 
@@ -197,19 +241,15 @@ static int contract_pair_impl(const qb_tensor_t *A, const int32_t *la,
                               void *workspace, size_t workspace_bytes,
                               void *stream) {
   PairPlan plan;
-  // QB_FORCE_CFG: tuning/debug override of the tile configuration
-  static const int force_cfg = [] {
-    const char *e = getenv("QB_FORCE_CFG");
-    return e ? atoi(e) : -1;
-  }();
   const bool ws_zeroed = (engine & QB_ENGINE_WS_ZEROED) != 0;
   engine &= 0xff;
-  int rc = plan_pair(A, la, B, lb, C, lc, conjA, conjB, plan, force_cfg);
+  int rc = plan_pair(A, la, B, lb, C, lc, conjA, conjB, plan, force_cfg());
   if (rc) return rc;
-  if ((rc = check_device_dtype(plan))) return rc;
+  const Route route = select_route(plan, engine);
+  if (route.kind == ROUTE_WIDEN) return check_device_dtype(plan);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (plan.empty_out) return 0;
-  if (plan.zero_fill) {
+  if (route.kind == ROUTE_EMPTY) return 0;
+  if (route.kind == ROUTE_ZERO_FILL) {
     if (beta == 0.0) return launch_fill_zero(C, st);
     if (beta == 1.0) return 0;
     set_error("zero-extent contraction with beta not in {0, 1}");
@@ -220,7 +260,7 @@ static int contract_pair_impl(const qb_tensor_t *A, const int32_t *la,
     static unsigned trace_launch = 0;  // 16 rotating slots of 8192 stamps
     plan.p.trace = tb + (size_t)(trace_launch++ % 16) * 8192;
   }
-  if (want_ozaki(engine, plan)) {
+  if (route.kind == ROUTE_INT8) {
     int64_t need = ozaki_workspace_bytes(plan) + kWsHeaderBytes;
     if (!workspace || (int64_t)workspace_bytes < need) {
       set_error("workspace too small: need %lld bytes, got %lld",
@@ -229,7 +269,7 @@ static int contract_pair_impl(const qb_tensor_t *A, const int32_t *la,
     }
     return launch_contract_ozaki(plan, static_cast<char *>(workspace) + kWsHeaderBytes, st);
   }
-  if (want_stream(engine, plan)) return launch_contract_stream(plan, st);
+  if (route.kind == ROUTE_STREAM) return launch_contract_stream(plan, st);
   int64_t need = plan_workspace_bytes(plan);
   if (need > 0) {
     if (!workspace || (int64_t)workspace_bytes < need) {

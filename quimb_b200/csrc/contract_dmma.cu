@@ -614,23 +614,8 @@ static int launch_cfg(const ContractParams &p, cudaStream_t st) {
   return launch_pdl(kern, grid, Cfg::NT, Cfg::SMEM, st, p);
 }
 
-// layout of the operand tiles in shared memory ([row][k] = "k-major"); for
-// real operands the big-tile kernels are specialised on it so that every
-// fragment address is base + immediate
-static inline int a_kmajor(const ContractParams &p) {
-  return (p.vecA == 2) || (p.vecA == 0 && p.thrA == 1);
-}
-static inline int b_kmajor(const ContractParams &p) {
-  return (p.vecB == 2) || (p.vecB == 0 && p.thrB == 1);
-}
-static inline bool layout_spec() {
-  static const bool on = [] {
-    const char *e = getenv("QB_LAYOUT_SPEC");
-    return e ? atoi(e) != 0 : true;
-  }();
-  return on;
-}
-
+// the cfg-0 kernels are specialised on the shared-memory layout of real
+// operands (a_kmajor / b_kmajor, plan.h); the route carries the choice
 template <bool CPLX, int LA, int LB, int BK = 16, int STAGES = 4>
 static int launch_streamk_l(const PairPlan &plan, cudaStream_t st) {
   using Cfg = KernelCfg<128, 128, BK, 4, 4, STAGES>;
@@ -648,10 +633,10 @@ static int launch_streamk_l(const PairPlan &plan, cudaStream_t st) {
 }
 
 template <bool CPLX>
-static int launch_streamk(const PairPlan &plan, cudaStream_t st) {
-  const bool bk32 = cfg0_bk() == 32;
-  if (!CPLX && layout_spec()) {
-    switch (a_kmajor(plan.p) * 2 + b_kmajor(plan.p) + (bk32 ? 4 : 0)) {
+static int launch_streamk(const PairPlan &plan, const Route &r, cudaStream_t st) {
+  const bool bk32 = r.bk == 32;
+  if (!CPLX && r.layout >= 0) {
+    switch (r.layout + (bk32 ? 4 : 0)) {
       case 0: return launch_streamk_l<false, 0, 0>(plan, st);
       case 1: return launch_streamk_l<false, 0, 1>(plan, st);
       case 2: return launch_streamk_l<false, 1, 0>(plan, st);
@@ -667,10 +652,10 @@ static int launch_streamk(const PairPlan &plan, cudaStream_t st) {
 }
 
 template <bool CPLX>
-static int launch_cfg0(const ContractParams &p, cudaStream_t st) {
+static int launch_cfg0(const ContractParams &p, const Route &r, cudaStream_t st) {
   if (!CPLX) {
-    if (layout_spec()) {
-      switch (a_kmajor(p) * 2 + b_kmajor(p) + (cfg0_bk() == 32 ? 4 : 0)) {
+    if (r.layout >= 0) {
+      switch (r.layout + (r.bk == 32 ? 4 : 0)) {
         case 0: return launch_cfg<128, 128, 16, 4, 4, 4, false, 0, 0>(p, st);
         case 1: return launch_cfg<128, 128, 16, 4, 4, 4, false, 0, 1>(p, st);
         case 2: return launch_cfg<128, 128, 16, 4, 4, 4, false, 1, 0>(p, st);
@@ -682,24 +667,25 @@ static int launch_cfg0(const ContractParams &p, cudaStream_t st) {
       }
     }
   }
-  if (cfg0_bk() == 32) return launch_cfg<128, 128, 32, 4, 4, 3, CPLX>(p, st);
+  if (r.bk == 32) return launch_cfg<128, 128, 32, 4, 4, 3, CPLX>(p, st);
   return launch_cfg<128, 128, 16, 4, 4, 4, CPLX>(p, st);
 }
 
 template <bool CPLX>
 static int launch_contract_t(const PairPlan &plan, cudaStream_t st) {
   const ContractParams &p = plan.p;
-  if (plan.streamk > 0 && p.partial) return launch_streamk<CPLX>(plan, st);
+  const Route r = dmma_route(plan, p.partial != nullptr);
+  if (r.kind == ROUTE_DMMA_STREAMK) return launch_streamk<CPLX>(plan, r, st);
   int rc;
-  switch (plan.cfg) {
-    case 0: rc = launch_cfg0<CPLX>(p, st); break;
+  switch (r.cfg) {
+    case 0: rc = launch_cfg0<CPLX>(p, r, st); break;
     case 1: rc = launch_cfg<64, 64, 16, 2, 2, 4, CPLX>(p, st); break;
     case 2: rc = launch_cfg<128, 32, 16, 4, 1, 4, CPLX>(p, st); break;
     case 3: rc = launch_cfg<32, 128, 16, 1, 4, 4, CPLX>(p, st); break;
     default: rc = launch_cfg<32, 32, 16, 2, 1, 4, CPLX>(p, st); break;
   }
   if (rc) return rc;
-  if (p.splitk > 1) {
+  if (r.splitk > 1) {
     int64_t total = p.M * p.N * p.nbatch * (CPLX ? 2 : 1);
     int blocks = (int)std::min<int64_t>((total + 255) / 256, (int64_t)sm_count() * 8);
     splitk_reduce_f64_kernel<CPLX><<<blocks, 256, 0, st>>>(p);

@@ -45,6 +45,17 @@
 //     (C_e[m, 2n+d] is the interleaved storage of complex C); the embedding is
 //     produced inside the split kernel's gather (conjugation = a sign there),
 //     so complex operands cost no extra pass either.
+//
+// Range and special values.  The exponents eA, eB stay integers: the split
+// kernel scales with ldexp(x, 6 - e) and the epilogue applies
+// ldexp(v * alpha, eA + eB - 12), so rows with a subnormal maximum and
+// products of huge rows with tiny columns neither overflow nor flush in an
+// intermediate.  A NaN counts as infinite in the row maximum, so a row or
+// column that holds a NaN or an infinity has a non-finite maximum: it gets
+// zero slices and the exponent kOzNonFinite, and the epilogue computes the
+// output elements of such rows and columns as plain fp64 dot products over
+// the original operands.  Their class (NaN, +inf, -inf) is then the one IEEE
+// arithmetic gives; finite inputs never take that branch.
 #include <cuda.h>
 #include <math.h>
 
@@ -172,29 +183,43 @@ struct SplitParams {
   int32_t S;
   int32_t k_contig;    // 1: consecutive k contiguous in memory, 0: rows
   unsigned long long *rowmax;  // [Rpad] max |x| as raw double bits
-  double *scale;               // [Rpad] 2^(e-6)
+  int32_t *expo;               // [Rpad] e: the row's slices carry x * 2^(6-e)
   int8_t *slices;              // [S][Rpad][Kpad]
 };
 
+// exponent of a row / column holding a NaN or an infinity: its slices are
+// zero and the GEMM epilogue computes its outputs directly in fp64
+constexpr int kOzNonFinite = 0x7fffffff;
+
 // element (r_e, k_e) of the real operand the GEMM sees: `off` = element offset
 // of the underlying (possibly complex) entry, d = r_e & 1, c = k_e & 1
-__device__ __forceinline__ double oz_load(const SplitParams &P, int64_t off, int d, int c) {
-  if (P.role == 0)
-    return P.single ? (double)static_cast<const float *>(P.src)[off]
-                    : static_cast<const double *>(P.src)[off];
+__device__ __forceinline__ double oz_elem(const void *src, int single, int role, int conj,
+                                          int64_t off, int d, int c) {
+  if (role == 0)
+    return single ? (double)static_cast<const float *>(src)[off]
+                  : static_cast<const double *>(src)[off];
   double re, im;
-  if (P.single) {
-    const float2 z = static_cast<const float2 *>(P.src)[off];
+  if (single) {
+    const float2 z = static_cast<const float2 *>(src)[off];
     re = z.x; im = z.y;
   } else {
-    const double2 z = static_cast<const double2 *>(P.src)[off];
+    const double2 z = static_cast<const double2 *>(src)[off];
     re = z.x; im = z.y;
   }
-  if (P.conj) im = -im;
-  if (P.role == 1) return c ? im : re;
+  if (conj) im = -im;
+  if (role == 1) return c ? im : re;
   // B-role: B_e[2k+c, 2n+d]
   if (c == d) return re;
   return c ? -im : im;
+}
+__device__ __forceinline__ double oz_load(const SplitParams &P, int64_t off, int d, int c) {
+  return oz_elem(P.src, P.single, P.role, P.conj, off, d, c);
+}
+// |x| for the row maximum; a NaN counts as infinite, so the maximum of a row
+// is finite exactly when every entry is (fmax alone would skip the NaN)
+__device__ __forceinline__ double oz_mag(double x) {
+  const double a = fabs(x);
+  return a == a ? a : (double)INFINITY;
 }
 
 __global__ void __launch_bounds__(256)
@@ -226,7 +251,7 @@ __global__ void __launch_bounds__(256)
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const int64_t ko = koff[tx + 32 * j];
-          if (ko >= 0) m = fmax(m, fabs(oz_load(P, ro + ko, (int)((r0 + r) & 1), (tx + 32 * j) & 1)));
+          if (ko >= 0) m = fmax(m, oz_mag(oz_load(P, ro + ko, (int)((r0 + r) & 1), (tx + 32 * j) & 1)));
         }
       }
 #pragma unroll
@@ -242,8 +267,8 @@ __global__ void __launch_bounds__(256)
       const int64_t ko = koff[ty + 8 * j];
       if (ko >= 0) {
         const int c = (ty + 8 * j) & 1;   // k0 is even
-        if (ro0 >= 0) m0 = fmax(m0, fabs(oz_load(P, ro0 + ko, tx & 1, c)));
-        if (ro1 >= 0) m1 = fmax(m1, fabs(oz_load(P, ro1 + ko, tx & 1, c)));
+        if (ro0 >= 0) m0 = fmax(m0, oz_mag(oz_load(P, ro0 + ko, tx & 1, c)));
+        if (ro1 >= 0) m1 = fmax(m1, oz_mag(oz_load(P, ro1 + ko, tx & 1, c)));
       }
     }
     red[ty][tx] = m0; red[ty][tx + 32] = m1;
@@ -263,25 +288,27 @@ __global__ void __launch_bounds__(256)
   __shared__ double tile[32][8 * 17];  // [row][k/16][16 + 1 pad]
   __shared__ int64_t roff[32];
   __shared__ int64_t koff[128];
-  __shared__ double inv_s[32];
+  __shared__ int sh_s[32];
   const int tid = threadIdx.x;
   const int64_t r0 = (int64_t)blockIdx.x * 32, k0 = (int64_t)blockIdx.y * 128;
   const int rsh = P.role == 2 ? 1 : 0, ksh = P.role != 0 ? 1 : 0;
   if (tid < 32) {
     const int64_t r = r0 + tid;
     int64_t o = -1, d;
-    double inv = 0.0;
+    int e = 0;
     if (r < P.R) {
-      decode2(r >> rsh, P.rows, o, d);
       const double mx = __longlong_as_double((long long)P.rowmax[r]);
-      int e = 0;
-      if (mx > 0.0) e = ilogb(mx) + 1;  // mx * 2^-e in [0.5, 1)
-      inv = ldexp(1.0, 6 - e);          // x * inv in (-64, 64)
-      if (blockIdx.y == 0) P.scale[r] = ldexp(1.0, e - 6);
-    } else if (blockIdx.y == 0) {
-      P.scale[r] = 0.0;
+      if (!isfinite(mx)) {
+        e = kOzNonFinite;  // zero slices (o stays -1)
+      } else {
+        decode2(r >> rsh, P.rows, o, d);
+        if (mx > 0.0) e = ilogb(mx) + 1;  // mx * 2^-e in [0.5, 1)
+      }
     }
-    roff[tid] = o; inv_s[tid] = inv;
+    if (blockIdx.y == 0) P.expo[r] = e;
+    // x * 2^(6-e) in (-64, 64), applied by ldexp: 2^(6-e) itself is not a
+    // double for rows whose maximum is below 2^-1017
+    roff[tid] = o; sh_s[tid] = 6 - e;
   }
   if (tid < 128) {
     const int64_t k = k0 + tid;
@@ -296,7 +323,7 @@ __global__ void __launch_bounds__(256)
     if (P.k_contig) { k = idx & 127; r = idx >> 7; } else { r = idx & 31; k = idx >> 5; }
     const int64_t ro = roff[r], ko = koff[k];
     double x = 0.0;
-    if (ro >= 0 && ko >= 0) x = oz_load(P, ro + ko, r & 1, k & 1) * inv_s[r];  // r0, k0 even
+    if (ro >= 0 && ko >= 0) x = ldexp(oz_load(P, ro + ko, r & 1, k & 1), sh_s[r]);  // r0, k0 even
     tile[r][(k >> 4) * 17 + (k & 15)] = x;
   }
   __syncthreads();
@@ -326,10 +353,31 @@ struct OzGemmParams {
   int32_t S;
   int32_t nkb;        // k-blocks of 128
   int32_t cplx;       // C is complex (interleaved): column 2n+d of the real GEMM
-  int64_t Me, Ne;     // extents of the real GEMM
-  const double *scaleA;   // [Mpad]
-  const double *scaleB;   // [Npad]
+  int64_t Me, Ne, Ke;     // extents of the real GEMM
+  const int32_t *expA;    // [Mpad] row exponents (kOzNonFinite: computed directly)
+  const int32_t *expB;    // [Npad] column exponents
 };
+
+// fp64 dot product of GEMM row m and column ne straight from the strided
+// operands (c.A, c.B through the m / n / k mode groups).  Only the outputs of
+// rows and columns that hold a NaN or an infinity take it, so they come out in
+// the class IEEE arithmetic gives (NaN, +inf or -inf).
+__device__ __noinline__ double oz_direct_dot(const OzGemmParams &P, int single, int64_t m,
+                                             int64_t ne) {
+  const ContractParams &c = P.c;
+  const int cplx = P.cplx;
+  int64_t oa, ob, t;
+  decode2(m, c.m, oa, t);
+  decode2(ne >> cplx, c.n, ob, t);
+  double s = 0.0;
+  for (int64_t k = 0; k < P.Ke; ++k) {
+    int64_t ka, kb;
+    decode2(k >> cplx, c.k, ka, kb);
+    s += oz_elem(c.A, single, cplx ? 1 : 0, c.conjA, oa + ka, 0, (int)(k & 1)) *
+         oz_elem(c.B, single, cplx ? 2 : 0, c.conjB, ob + kb, (int)(ne & 1), (int)(k & 1));
+  }
+  return s;
+}
 
 // BN output columns per CTA, NSL accumulators (the most slices the
 // instantiation takes): NSL x BN/2 = 128 accumulator registers per consumer
@@ -362,8 +410,8 @@ __global__ void __launch_bounds__(OZ_THREADS, 1)
   uint64_t *emptyB = fullB + 2;                               // [2]
   int64_t *offCm = reinterpret_cast<int64_t *>(aux + 256);    // [128]
   int64_t *offCn = offCm + OZ_BM;                             // [BN]
-  double *sclM = reinterpret_cast<double *>(offCn + BN);      // [128]
-  double *sclN = sclM + OZ_BM;                                // [BN]
+  int32_t *expM = reinterpret_cast<int32_t *>(offCn + BN);    // [128]
+  int32_t *expN = expM + OZ_BM;                               // [BN]
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int S = P.S, nkb = P.nkb;
@@ -389,14 +437,14 @@ __global__ void __launch_bounds__(OZ_THREADS, 1)
       int64_t oa, oc = -1;
       if (m < P.Me) { decode2(m, P.c.m, oa, oc); oc <<= csh; }
       offCm[e] = oc;
-      sclM[e] = P.scaleA[(int64_t)tm * OZ_BM + e];
+      expM[e] = P.expA[(int64_t)tm * OZ_BM + e];
     } else if (e - OZ_BM < BN) {
       const int c = e - OZ_BM;
       const int64_t ne = (int64_t)tn * BN + c;
       int64_t ob, oc = -1;
       if (ne < P.Ne) { decode2(ne >> csh, P.c.n, ob, oc); oc = (oc << csh) + (csh ? (ne & 1) : 0); }
       offCn[c] = oc;
-      sclN[c] = P.scaleB[(int64_t)tn * BN + c];
+      expN[c] = P.expB[(int64_t)tn * BN + c];
     }
   }
   __syncthreads();
@@ -476,15 +524,17 @@ __global__ void __launch_bounds__(OZ_THREADS, 1)
 
   // ============================== epilogue ================================
   // combine the S accumulators in fp64 with exact power-of-two weights,
-  // apply the row / column scales and alpha/beta, scatter to the strided C
+  // apply alpha and the row / column scales 2^(eA + eB - 12) in one ldexp (no
+  // intermediate can overflow or underflow), add beta C, scatter to the
+  // strided C
   OutT *C = static_cast<OutT *>(P.c.C);
-  const double beta = P.c.beta;
+  const double alpha = P.c.alpha, beta = P.c.beta;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int row = half * 64 + wq * 16 + (lane >> 2) + 8 * h;
     const int64_t om = offCm[row];
     if (om < 0) continue;
-    const double sm = sclM[row] * P.c.alpha;
+    const int eM = expM[row];
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
@@ -501,7 +551,13 @@ __global__ void __launch_bounds__(OZ_THREADS, 1)
         }
         const int64_t on = offCn[col];
         if (on >= 0) {
-          double val = v * sm * sclN[col];
+          const int eN = expN[col];
+          double val;
+          if (eM == kOzNonFinite || eN == kOzNonFinite)
+            val = alpha * oz_direct_dot(P, sizeof(OutT) == 4, (int64_t)tm * OZ_BM + row,
+                                        (int64_t)tn * BN + col);
+          else
+            val = ldexp(v * alpha, eM + eN - 12);
           if (beta != 0.0) val += beta * (double)C[om + on];
           C[om + on] = (OutT)val;
         }
@@ -655,7 +711,7 @@ int launch_contract_ozaki(const PairPlan &plan, void *workspace, cudaStream_t st
     const int64_t ksm = ks.n ? sp.ks.s0[0] : 1, rsm = rows.n ? sp.rows.s0[0] : (int64_t)1 << 60;
     sp.k_contig = (ksm <= rsm) ? 1 : 0;
     sp.rowmax = reinterpret_cast<unsigned long long *>(ws + off_rm);
-    sp.scale = reinterpret_cast<double *>(ws + off_sc);
+    sp.expo = reinterpret_cast<int32_t *>(ws + off_sc);
     sp.slices = reinterpret_cast<int8_t *>(ws + off_sl);
     dim3 g1((unsigned)((R + 63) / 64), (unsigned)((g.Ke + 255) / 256));
     ozaki_rowmax_kernel<<<g1, 256, 0, st>>>(sp);
@@ -687,9 +743,9 @@ int launch_contract_ozaki(const PairPlan &plan, void *workspace, cudaStream_t st
   gp.S = g.S;
   gp.nkb = (int)(g.Kpad / OZ_BK);
   gp.cplx = g.cplx;
-  gp.Me = g.Me; gp.Ne = g.Ne;
-  gp.scaleA = reinterpret_cast<const double *>(ws + g.off_scA);
-  gp.scaleB = reinterpret_cast<const double *>(ws + g.off_scB);
+  gp.Me = g.Me; gp.Ne = g.Ne; gp.Ke = g.Ke;
+  gp.expA = reinterpret_cast<const int32_t *>(ws + g.off_scA);
+  gp.expB = reinterpret_cast<const int32_t *>(ws + g.off_scB);
   dim3 grid((unsigned)(g.Mpad / OZ_BM), (unsigned)((g.Ne + g.BN - 1) / g.BN));
   if (g.single) return oz_launch_gemm<OZ_BN_SINGLE, OZ_MAXS_SINGLE, float>(mapA, mapB, gp, grid, st);
   return oz_launch_gemm<OZ_BN_DOUBLE, OZ_MAXS, double>(mapA, mapB, gp, grid, st);

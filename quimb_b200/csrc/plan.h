@@ -411,6 +411,64 @@ inline int plan_pair(const qb_tensor_t *A, const int32_t *la,
   return 0;
 }
 
+// layout of the operand tiles in shared memory ([row][k] = "k-major"); for
+// real operands the large-tile kernels are specialised on it so that every
+// fragment address is base + immediate
+inline int a_kmajor(const ContractParams &p) {
+  return (p.vecA == 2) || (p.vecA == 0 && p.thrA == 1);
+}
+inline int b_kmajor(const ContractParams &p) {
+  return (p.vecB == 2) || (p.vecB == 0 && p.thrB == 1);
+}
+inline bool layout_spec() {
+  static const bool on = [] {
+    const char *e = getenv("QB_LAYOUT_SPEC");
+    return e ? atoi(e) != 0 : true;
+  }();
+  return on;
+}
+
+// Which kernel a contraction runs.  select_route (api.cu) decides the engine;
+// dmma_route fills in the DMMA details.  The launchers read the same fields,
+// so qb_contract_pair_route reports exactly what qb_contract_pair runs.
+enum RouteKind {
+  ROUTE_EMPTY = 0,         // output has no elements: nothing runs
+  ROUTE_ZERO_FILL = 1,     // contracted extent 0: C = 0 (beta = 0)
+  ROUTE_WIDEN = 2,         // single precision below the int8 engine's minimum
+  ROUTE_INT8 = 3,          // int8 error-free-split engine (ozaki_tc.cu)
+  ROUTE_STREAM = 4,        // streaming engine (contract_stream.cu)
+  ROUTE_DMMA = 5,          // DMMA tile kernel, classic grid (+ split-K reduce)
+  ROUTE_DMMA_STREAMK = 6,  // DMMA large tile, persistent stream-K grid
+};
+struct Route {
+  int kind;
+  int cfg;        // DMMA tile configuration, -1 otherwise
+  int splitk;     // split-K factor (1: none)
+  int streamk;    // stream-K grid (CTAs), 0 otherwise
+  int sk_head;    // stream-K cost of a tile's fix-up, in k-blocks
+  int bk;         // DMMA k-block depth
+  int layout;     // cfg 0, real: a_kmajor * 2 + b_kmajor; -1: runtime layout
+  int launches;   // kernels launched (beta = 0)
+};
+
+// DMMA part of a route.  A stream-K grid needs the workspace scratch that the
+// planner sized for it (internal GEMMs without scratch run classic launches).
+inline Route dmma_route(const PairPlan &plan, bool have_scratch) {
+  Route r{ROUTE_DMMA, plan.cfg, plan.p.splitk, 0, 0, tile_cfg(plan.cfg).bk, -1, 1};
+  const bool cplx = dtype_is_complex(plan.dtype);
+  if (plan.streamk > 0 && have_scratch) {
+    r.kind = ROUTE_DMMA_STREAMK;
+    r.splitk = 1;
+    r.streamk = plan.streamk;
+    r.sk_head = plan.p.sk_head;
+  } else if (r.splitk > 1) {
+    r.launches = 2;  // + splitk_reduce_f64_kernel
+  }
+  if (plan.cfg == 0 && !cplx && layout_spec())
+    r.layout = a_kmajor(plan.p) * 2 + b_kmajor(plan.p);
+  return r;
+}
+
 // scratch for partial sums (stream-K parked tiles / split-K partial outputs)
 inline int64_t plan_scratch_bytes(const PairPlan &plan) {
   if (plan.streamk > 0)

@@ -34,7 +34,7 @@ _REAL = {_lib.QB_F32: np.float32, _lib.QB_F64: np.float64,
          _lib.QB_C64: np.float32, _lib.QB_C128: np.float64}
 
 _HOST_ONLY = {
-    "qb_abi_version", "qb_last_error", "qb_contract_pair_plan",
+    "qb_abi_version", "qb_last_error", "qb_contract_pair_plan", "qb_contract_pair_route",
     "qb_contract_pair_workspace", "qb_dot_workspace", "qb_multi_dot_workspace",
     "qb_qr_workspace", "qb_svd_workspace", "qb_svals_to_keep",
 }

@@ -9,6 +9,7 @@ import torch
 
 import quimb_b200 as qb
 from oracle import contract_np as cn
+from tests import route_oracle as ro
 
 pytestmark = pytest.mark.gpu
 
@@ -115,6 +116,18 @@ CASES = [
 ]
 
 
+def _elementwise_bound(eq, sizes, a, b):
+    """|C_kernel - C_numpy| <= 2 gamma_K (|A|.|B|) element by element (complex:
+    2 sqrt(2) gamma_{2K+2}), K = number of summed terms: both results are
+    inner products in some summation order (route_oracle.dmma_bound)."""
+    lhs, rhs = eq.split("->")
+    K = int(np.prod([sizes[c] for c in set(lhs.replace(",", "")) if c not in rhs]))
+    absref = np.einsum(eq, np.abs(a), np.abs(b))
+    if np.iscomplexobj(a):
+        return 2 * np.sqrt(2) * ro.gamma(2 * K + 2) * absref * 1.001
+    return 2 * ro.gamma(K) * absref * 1.001
+
+
 @pytest.mark.parametrize("dtype", ["float64", "complex128"])
 @pytest.mark.parametrize("eq,sizes", CASES)
 def test_pairwise_vs_oracle(eq, sizes, dtype):
@@ -124,8 +137,9 @@ def test_pairwise_vs_oracle(eq, sizes, dtype):
     a = _rand(rng, [sizes[c] for c in ta], dtype)
     b = _rand(rng, [sizes[c] for c in tb], dtype)
     ref = np.einsum(eq, a, b)
-    out = qb.einsum(eq, qb.asarray(a), qb.asarray(b))
-    _close(out.to_numpy(), ref, 1e-11)
+    out = qb.einsum(eq, qb.asarray(a), qb.asarray(b)).to_numpy()
+    assert out.shape == ref.shape
+    assert np.all(np.abs(out - ref) <= _elementwise_bound(eq, sizes, a, b))
 
 
 def test_oracle_pair_executor_agrees():
@@ -240,7 +254,7 @@ OZ_CASES = [
 
 
 @pytest.mark.parametrize("eq,sizes", OZ_CASES)
-def test_tcgen05_engine_matches_oracle(eq, sizes):
+def test_int8_engine_matches_oracle(eq, sizes):
     rng = np.random.default_rng(abs(hash(eq)) % 2**31)
     lhs, rhs = eq.split("->")
     ta, tb = lhs.split(",")
@@ -258,7 +272,7 @@ def test_tcgen05_engine_matches_oracle(eq, sizes):
     assert np.max(np.abs(out.cpu().numpy() - ref)) <= 1e-12 * np.max(np.abs(ref))
 
 
-def test_tcgen05_engine_badly_scaled_and_accumulate():
+def test_int8_engine_badly_scaled_and_accumulate():
     rng = np.random.default_rng(8)
     a = rng.standard_normal((256, 384)) * np.logspace(-9, 9, 256)[:, None]
     b = rng.standard_normal((384, 192)) * np.logspace(-7, 7, 192)[None, :]
@@ -372,7 +386,7 @@ def test_native_single_accumulate_and_strided_output():
     assert np.max(np.abs(C.to_numpy().T - ref)) <= 3e-6 * np.max(np.abs(ref))
 
 
-def test_tcgen05_engine_complex128_embedding():
+def test_int8_engine_complex128_embedding():
     """complex128 through the same engine (8 slices): the complex operands are
     embedded into the real GEMM inside the split gather."""
     rng = np.random.default_rng(22)
@@ -381,3 +395,111 @@ def test_tcgen05_engine_complex128_embedding():
                            conj_a=True, engine=2)
     ref = np.einsum("abc,cbd->da", a.conj(), b)
     assert np.max(np.abs(out.cpu().numpy() - ref)) <= 1e-12 * np.max(np.abs(ref))
+
+
+# ---- int8 engine edges: ragged tiles, the K limit, special values, range ----
+_INT8_DTYPES = ["float32", "complex64", "float64", "complex128"]
+
+
+def _int8_engine(dtype):
+    # float32 / complex64 take it by default, float64 / complex128 on request
+    return ro.ENGINE_INT8 if dtype in ("float64", "complex128") else 0
+
+
+def _int8_route(M, K, N, dtype):
+    return ro.route_of("ab,bc", M, K, N, dtype, _int8_engine(dtype))
+
+
+def _run_int8(a, b, dtype, **kw):
+    out = qb.contract_pair(torch.from_numpy(a).cuda(), [0, 1], torch.from_numpy(b).cuda(),
+                           [1, 2], [0, 2], engine=_int8_engine(dtype), **kw)
+    return out.cpu().numpy()
+
+
+def _ragged_cases():
+    for dtype in _INT8_DTYPES:
+        ns = (32, 33) if dtype.startswith("complex") else (64, 65, 97)
+        for M, N, K in itertools.product((128, 129, 255), ns, (128, 129, 255)):
+            yield dtype, M, N, K
+
+
+@pytest.mark.parametrize("dtype,M,N,K", list(_ragged_cases()))
+def test_int8_engine_ragged_edges(dtype, M, N, K):
+    """Extents around the 128-row tile, the output-column tile (64 float32 /
+    32 float64 real columns; complex columns count twice) and the 128-byte
+    k-block: exact on integer inputs, within the engine's bound on normal ones."""
+    assert _int8_route(M, K, N, dtype)["kind"] == "int8"
+    rng = np.random.default_rng(M * 7919 + N * 31 + K)
+    a, b = ro.int_operand(rng, (M, K), dtype), ro.int_operand(rng, (K, N), dtype)
+    np.testing.assert_array_equal(_run_int8(a, b, dtype), (ro.wide(a) @ ro.wide(b)).astype(dtype))
+    a, b = ro.normal_operand(rng, (M, K), dtype), ro.normal_operand(rng, (K, N), dtype)
+    got = ro.wide(_run_int8(a, b, dtype))
+    bound = ro.int8_bound(a, b, dtype in ("float32", "complex64"))
+    assert np.all(np.abs(got - ro.wide(a) @ ro.wide(b)) <= bound)
+
+
+@pytest.mark.parametrize("dtype", ["float64", "float32"])
+def test_int8_engine_k_limit(dtype):
+    """K = 65535 is the largest contracted extent whose int32 sums are proven
+    exact; entries of magnitude 1 - 2^-8 (just below a power of two) make every
+    first slice +-64 and the first accumulator of an all-positive row / column
+    reach 65535 * 4096.  Exact oracle: the products have 17 significant bits
+    and every partial sum stays below 2^16, so float64 numpy is exact.
+    K = 65536 leaves the engine (float64: DMMA; float32: widened)."""
+    M, N = 128, 64
+    rng = np.random.default_rng(65535)
+    for K, kind in ((65535, "int8"), (65536, "dmma" if dtype == "float64" else "widen")):
+        assert _int8_route(M, K, N, dtype)["kind"] == kind
+        v = 1.0 - 2.0 ** -8
+        a = rng.choice([-v, v], size=(M, K))
+        b = rng.choice([-v, v], size=(K, N))
+        a[0], b[:, 0] = v, v
+        ref = a @ b
+        assert ref[0, 0] == K * v * v
+        got = _run_int8(a.astype(dtype), b.astype(dtype), dtype)
+        np.testing.assert_array_equal(got, ref.astype(dtype))
+
+
+@pytest.mark.parametrize("dtype", _INT8_DTYPES)
+def test_int8_engine_nonfinite_inputs(dtype):
+    """NaN, +inf and -inf in A and B: the int8 slices cannot hold them, so the
+    rows and columns that contain them are computed directly; every output
+    element is in the IEEE class of the exact result and the finite ones keep
+    the engine's bound."""
+    M, K = 130, 200
+    N = 40 if dtype.startswith("complex") else 70
+    assert _int8_route(M, K, N, dtype)["kind"] == "int8"
+    rng = np.random.default_rng(404)
+    a, b = ro.plant_nonfinite(ro.normal_operand(rng, (M, K), dtype),
+                              ro.normal_operand(rng, (K, N), dtype))
+    got = ro.wide(_run_int8(a, b, dtype))
+    ro.check_classes(a[None], b[None], got[None], int8=True)
+
+
+def test_int8_engine_extreme_exponents():
+    """float64 on the int8 engine across the exponent range: rows whose maximum
+    is subnormal (2^-1030 ~ 1e-310) against columns near 2^1000, rows near
+    2^1020 (~1e307) against columns near 2^-1020, all-zero rows and columns.
+    Where the exact result is a normal number it meets the engine's bound;
+    zero rows and columns give 0."""
+    M, K, N = 130, 256, 70
+    assert _int8_route(M, K, N, "float64")["kind"] == "int8"
+    rng = np.random.default_rng(1015)
+    ea = np.zeros(M, dtype=int)
+    ea[:20], ea[20:40] = -1030, 1020
+    eb = np.zeros(N, dtype=int)
+    eb[:15], eb[15:30], eb[30:40] = -1020, 1000, -40
+    a = np.ldexp(rng.standard_normal((M, K)), ea[:, None])
+    b = np.ldexp(rng.standard_normal((K, N)), eb[None, :])
+    a[40], b[:, 40] = 0.0, 0.0
+    # the exact product of the inputs as given (subnormal rows keep fewer bits)
+    a1, b1 = np.ldexp(a, -ea[:, None]), np.ldexp(b, -eb[None, :])
+    with np.errstate(over="ignore"):     # results beyond the double range are not checked
+        ref = np.ldexp(a1 @ b1, ea[:, None] + eb[None, :])
+        bound = np.ldexp(ro.int8_bound(a1[None], b1[None], False)[0], ea[:, None] + eb[None, :])
+    got = _run_int8(a, b, "float64")
+    normal = np.isfinite(ref) & (np.abs(ref) >= np.finfo(np.float64).tiny)
+    normal &= np.isfinite(bound)
+    assert normal[:20].any() and normal[20:40, :15].all()
+    assert np.all(np.abs(got[normal] - ref[normal]) <= bound[normal])
+    assert np.all(got[40] == 0.0) and np.all(got[:, 40] == 0.0)

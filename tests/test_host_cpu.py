@@ -296,6 +296,97 @@ def test_planner_diagonal_and_summed_labels():
         qb.plan_pair([4, 5], [5, 1], [0, 0], [], [], [], [4], [1], [0])
 
 
+def _route(sa, la, sb, lb, sc, lc, dtype=_lib.QB_F64, engine=0):
+    return qb.route_pair(sa, _strides(sa), la, sb, _strides(sb), lb, sc, _strides(sc), lc,
+                         dtype, engine)
+
+
+def test_route_report_engines():
+    """qb_contract_pair_route: one decision for every engine."""
+    r = _route([0, 4], [0, 1], [4, 3], [1, 2], [0, 3], [0, 2])
+    assert r["kind"] == "empty" and r["launches"] == 0
+    r = _route([3, 0], [0, 1], [0, 2], [1, 2], [3, 2], [0, 2])
+    assert r["kind"] == "zero_fill" and r["launches"] == 1
+    # single precision: int8 engine above its minimum, widened below it
+    assert _route([128, 128], [0, 1], [128, 64], [1, 2], [128, 64], [0, 2],
+                  _lib.QB_F32)["kind"] == "int8"
+    assert _route([127, 128], [0, 1], [128, 64], [1, 2], [127, 64], [0, 2],
+                  _lib.QB_F32)["kind"] == "widen"
+    # float64: the int8 engine only on request (5 launches), streaming engine
+    # for small operators only on request
+    sq = ([256, 256], [0, 1], [256, 256], [1, 2], [256, 256], [0, 2])
+    assert _route(*sq)["kind"] == "dmma"
+    r = _route(*sq, engine=_lib.QB_ENGINE_OZAKI)
+    assert r["kind"] == "int8" and r["launches"] == 5
+    small = ([4096, 8], [0, 1], [8, 8], [1, 2], [4096, 8], [0, 2])
+    assert _route(*small, engine=_lib.QB_ENGINE_STREAM)["kind"] == "stream"
+    assert _route(*small)["kind"] == "dmma"
+    # split-K launches the reduction kernel too
+    r = _route([130, 4096], [0, 1], [4096, 130], [1, 2], [130, 130], [0, 2])
+    assert r["kind"] == "dmma" and r["splitk"] > 1 and r["launches"] == 2
+    # the K limit of the int8 engine: f K < 65536 real units
+    kl = lambda K, dt: _route([128, K], [0, 1], [K, 64], [1, 2], [128, 64], [0, 2], dt,  # noqa: E731
+                              _lib.QB_ENGINE_OZAKI)["kind"]
+    assert kl(65535, _lib.QB_F64) == "int8" and kl(65536, _lib.QB_F64) == "dmma"
+    assert kl(65535, _lib.QB_F32) == "int8" and kl(65536, _lib.QB_F32) == "widen"
+    assert kl(32767, _lib.QB_C64) == "int8" and kl(32768, _lib.QB_C64) == "widen"
+
+
+def test_route_pinned_for_baseline_shapes():
+    """The routes of the BASELINE shapes at the H100 SXM's 132 SMs (the count
+    the planner assumes without a device): a planner change shows up here."""
+    chi, d, w = 1024, 2, 5
+    r = _route([chi, chi], [0, 1], [chi, d, chi], [1, 2, 3], [chi, d, chi], [0, 2, 3])
+    if r["sms"] != 132:
+        pytest.skip(f"this device has {r['sms']} SMs; the pinned routes are for 132")
+    big = dict(cfg=0, splitk=1, bk=32, sms=132, launches=1)
+    # MPS norm (bench): ket step E[a, b] A[b, p, b'] -- 128 tiles fill 132 SMs
+    # well enough for the classic launch
+    assert r == dict(kind="dmma", streamk=0, sk_head=0, layout=2, **big)
+    # bra step A[a, p, a'] T[a, p, b']: stream-K, both operands [k][row]
+    r = _route([chi, d, chi], [0, 1, 2], [chi, d, chi], [0, 1, 3], [chi, chi], [2, 3])
+    assert r == dict(kind="dmma_streamk", streamk=132, sk_head=4, layout=0, **big)
+    # DMRG L . x (5120 x 1024 x 4096)
+    r = _route([chi, w, chi], [0, 1, 2], [chi, d, d, chi], [2, 3, 4, 5], [chi, w, d, d, chi],
+               [0, 1, 3, 4, 5])
+    assert r == dict(kind="dmma", streamk=0, sk_head=0, layout=2, **big)
+    # 4096^3
+    n = 4096
+    r = _route([n, n], [0, 1], [n, n], [1, 2], [n, n], [0, 2])
+    assert r == dict(kind="dmma", streamk=0, sk_head=0, layout=2, **big)
+
+
+def test_route_search_reaches_every_route():
+    """The GPU route matrix (tests/test_gpu_routes.py) finds a grid shape for
+    every route; here at the SM count the planner sees on this machine."""
+    from tests import route_oracle as ro
+    found = ro.search_routes()
+    missing = ro.required_keys() - set(found)
+    assert not missing, sorted(missing, key=str)
+    assert max(ro.macs(*v[:4], k[0]) for k, v in found.items()) <= ro.MAX_MACS
+
+
+def test_nonfinite_class_oracle_matches_numpy():
+    """The class oracle of the route tests agrees with numpy's own
+    element-by-element arithmetic (einsum without BLAS)."""
+    import warnings
+    from tests import route_oracle as ro
+    rng = np.random.default_rng(0)
+    for dt in ("float64", "complex128"):
+        a, b = ro.plant_nonfinite(ro.normal_operand(rng, (9, 7), dt),
+                                  ro.normal_operand(rng, (7, 6), dt))
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            ref = np.einsum("ab,bc->ac", a, b, optimize=False)
+        cls = ro.nonfinite_class(a, b)
+        if dt == "complex128":
+            np.testing.assert_array_equal(cls[0], ro.classify(ref.real))
+            np.testing.assert_array_equal(cls[1], ro.classify(ref.imag))
+        else:
+            np.testing.assert_array_equal(cls, ro.classify(ref))
+            assert set(np.unique(cls)) == {0, 1, 2, 3}
+
+
 def test_svd_trunc_and_p2p_argument_errors_without_a_device():
     """Argument checks of the new entry points run before any CUDA call."""
     import ctypes
