@@ -61,11 +61,15 @@ __device__ __forceinline__ void load_tile(
   // smem layout: vec==1 or (vec==0 && thr==0) -> [k][row]; else [row][k]
   // KM >= 0: the layout is a compile-time constant (specialised kernels)
   const bool kmajor = KM >= 0 ? (KM == 1) : ((vec == 2) || (vec == 0 && thr == 1));
+  // the 8-warp 128x128 tile issues up to 16 copies per thread; unrolled in
+  // full, ptxas keeps the index arithmetic of all of them live across the
+  // k-loop and spills
+  constexpr int UNROLL = NT >= 256 ? 4 : 16;
   const int s_row = kmajor ? (BK + 4) : 1;
   const int s_k = kmajor ? 1 : (ROWS + 4);
   if (vec == 0) {
     constexpr int TOTAL = ROWS * BK;
-#pragma unroll
+#pragma unroll UNROLL
     for (int c0 = 0; c0 < TOTAL; c0 += NT) {
       int c = c0 + tid;
       if (TOTAL % NT != 0 && c >= TOTAL) break;
@@ -79,7 +83,7 @@ __device__ __forceinline__ void load_tile(
   } else if (vec == 2) {
     constexpr int TOTAL = ROWS * BK / 2;
     constexpr int KC = BK / 2;
-#pragma unroll
+#pragma unroll UNROLL
     for (int c0 = 0; c0 < TOTAL; c0 += NT) {
       int c = c0 + tid;
       if (TOTAL % NT != 0 && c >= TOTAL) break;
@@ -94,7 +98,7 @@ __device__ __forceinline__ void load_tile(
   } else {
     constexpr int TOTAL = ROWS * BK / 2;
     constexpr int RC = ROWS / 2;
-#pragma unroll
+#pragma unroll UNROLL
     for (int c0 = 0; c0 < TOTAL; c0 += NT) {
       int c = c0 + tid;
       if (TOTAL % NT != 0 && c >= TOTAL) break;
@@ -117,7 +121,8 @@ __device__ __forceinline__ void load_tile_cplx(
     const int64_t *__restrict__ n_off, const int64_t *__restrict__ k_off,
     int thr, int tid) {
   constexpr int TOTAL = NC * KC;
-#pragma unroll
+  constexpr int UNROLL = NT >= 256 ? 4 : 16;  // as in load_tile
+#pragma unroll UNROLL
   for (int c0 = 0; c0 < TOTAL; c0 += NT) {
     int c = c0 + tid;
     if (TOTAL % NT != 0 && c >= TOTAL) break;
@@ -618,8 +623,8 @@ static int launch_cfg(const ContractParams &p, cudaStream_t st) {
 // operands (a_kmajor / b_kmajor, plan.h); the route carries the choice
 template <bool CPLX, int LA, int LB, int BK = 16, int STAGES = 4>
 static int launch_streamk_l(const PairPlan &plan, cudaStream_t st) {
-  using Cfg = KernelCfg<128, 128, BK, 4, 4, STAGES>;
-  auto kern = contract_f64_streamk_kernel<128, 128, BK, 4, 4, STAGES, CPLX, LA, LB>;
+  using Cfg = KernelCfg<128, 128, BK, 2, 4, STAGES>;
+  auto kern = contract_f64_streamk_kernel<128, 128, BK, 2, 4, STAGES, CPLX, LA, LB>;
   static bool attr_set = false;
   if (!attr_set) {
     QB_CUDA_CHECK(cudaFuncSetAttribute(
@@ -656,19 +661,19 @@ static int launch_cfg0(const ContractParams &p, const Route &r, cudaStream_t st)
   if (!CPLX) {
     if (r.layout >= 0) {
       switch (r.layout + (r.bk == 32 ? 4 : 0)) {
-        case 0: return launch_cfg<128, 128, 16, 4, 4, 4, false, 0, 0>(p, st);
-        case 1: return launch_cfg<128, 128, 16, 4, 4, 4, false, 0, 1>(p, st);
-        case 2: return launch_cfg<128, 128, 16, 4, 4, 4, false, 1, 0>(p, st);
-        case 3: return launch_cfg<128, 128, 16, 4, 4, 4, false, 1, 1>(p, st);
-        case 4: return launch_cfg<128, 128, 32, 4, 4, 3, false, 0, 0>(p, st);
-        case 5: return launch_cfg<128, 128, 32, 4, 4, 3, false, 0, 1>(p, st);
-        case 6: return launch_cfg<128, 128, 32, 4, 4, 3, false, 1, 0>(p, st);
-        default: return launch_cfg<128, 128, 32, 4, 4, 3, false, 1, 1>(p, st);
+        case 0: return launch_cfg<128, 128, 16, 2, 4, 4, false, 0, 0>(p, st);
+        case 1: return launch_cfg<128, 128, 16, 2, 4, 4, false, 0, 1>(p, st);
+        case 2: return launch_cfg<128, 128, 16, 2, 4, 4, false, 1, 0>(p, st);
+        case 3: return launch_cfg<128, 128, 16, 2, 4, 4, false, 1, 1>(p, st);
+        case 4: return launch_cfg<128, 128, 32, 2, 4, 3, false, 0, 0>(p, st);
+        case 5: return launch_cfg<128, 128, 32, 2, 4, 3, false, 0, 1>(p, st);
+        case 6: return launch_cfg<128, 128, 32, 2, 4, 3, false, 1, 0>(p, st);
+        default: return launch_cfg<128, 128, 32, 2, 4, 3, false, 1, 1>(p, st);
       }
     }
   }
-  if (r.bk == 32) return launch_cfg<128, 128, 32, 4, 4, 3, CPLX>(p, st);
-  return launch_cfg<128, 128, 16, 4, 4, 4, CPLX>(p, st);
+  if (r.bk == 32) return launch_cfg<128, 128, 32, 2, 4, 3, CPLX>(p, st);
+  return launch_cfg<128, 128, 16, 2, 4, 4, CPLX>(p, st);
 }
 
 template <bool CPLX>

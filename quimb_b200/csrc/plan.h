@@ -108,7 +108,7 @@ struct TileCfg {
   int bm, bn, bk, threads;
 };
 static const TileCfg kTileCfgs[] = {
-    {128, 128, 16, 512},  // 0: large
+    {128, 128, 16, 256},  // 0: large
     {64, 64, 16, 128},    // 1: medium
     {128, 32, 16, 128},   // 2: tall (small N)
     {32, 128, 16, 128},   // 3: wide (small M)

@@ -89,7 +89,7 @@ if __name__ == "__main__":
     full(f"prof_contract_{TAG}.ncu-rep", f"{TAG}_contract_kernel_ncu_full.txt", [
         f"# ncu --set full --clock-control none --import-source on -k regex:contract_f64_streamk -s 1000 -c 2 "
         "(bench.py: MPS norm L=200 chi=1024 fp64)",
-        "# persistent stream-K launch of the 128x128x32 (3-stage, 16 warps, compile-time tile layouts) DMMA",
+        "# persistent stream-K launch of the 128x128x32 (3-stage, 8 warps, compile-time tile layouts) DMMA",
         "# contraction kernel, 148 CTAs, programmatic dependent launch",
         "# launch 1: E[a',a].A[a,(b,p)]  M=1024 N=2048 K=1024;  launch 2: conj(A)[(a',p),b'].T  M=N=1024 K=2048",
         "# algorithmic per launch: 4.295 GFLOP, 33.5 MB (fp64) -> tensor bound; DMMA peak measured 37.16 TFLOP/s"])
