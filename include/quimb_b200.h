@@ -258,6 +258,15 @@ int qb_qr_stab(int dtype, int64_t m, int64_t n, const void *X, void *Q,
                void *R, int stabilized, void *workspace,
                size_t workspace_bytes, void *stream);
 int64_t qb_qr_workspace(int dtype, int64_t m, int64_t n);
+/* Host only: the kernels qb_qr_stab launches for an m x n matrix, from the
+ * decisions of the launch path.  out[0] = inner panel width, out[1] = outer
+ * (aggregated) panel width, out[2] = outer panels, out[3] = bitmask of the
+ * panel instantiations launched (bit 0: (32 columns, 1 row per thread),
+ * 1: (32, 2), 2: (16, 4), 3: (8, 8)), out[4] = 1 when wy_t_kernel forms the
+ * aggregated T factors, out[5] = inner panels.  The caller provides 16 slots.
+ * qb_qr_stab and the SVD factor 2^-e X when max|X| lies outside
+ * [2^-200, 2^200] (e = ilogb(max|X|)) and scale the results back. */
+int qb_qr_route(int64_t m, int64_t n, int64_t *out16);
 
 /*
  * Thin SVD of a row-major contiguous m x n matrix X by one-sided block
@@ -296,6 +305,19 @@ int qb_svd_trunc(int dtype, int64_t m, int64_t n, const void *X, double cutoff,
                  void *U, void *S, void *VH, int64_t *n_keep,
                  double *trunc_error, int64_t *n_null, void *workspace,
                  size_t workspace_bytes, int *sweeps_out, void *stream);
+/* qb_svd / qb_svd_trunc return -9 (before any Jacobi sweep) when X holds a
+ * NaN or an infinity. */
+
+/* Host only: what qb_svd_trunc launches for a tall m x n matrix (m >= n) and
+ * absorb mode (qb_svd: QB_ABSORB_FULL), from the decisions of the launch
+ * path.  out[0] = padded column count, out[1] = column blocks, out[2] =
+ * independent stream groups of a sweep, out[3] = cluster size, out[4] = rows
+ * per streamed chunk, out[5] = cp.async stages, out[6] = epilogue (0
+ * accumulated rotations, 1 left family, 2 right family, 3 values only),
+ * out[7] = sweeps that may replay the cached sweep graph (0: none),
+ * out[8] / out[9] = panel mask / wy_t of the QR preconditioner (as
+ * qb_qr_route), out[10] = round launches per sweep.  16 slots. */
+int qb_svd_route(int64_t m, int64_t n, int absorb, int64_t *out16);
 
 /*
  * Host-side truncation rule of svd_truncated's numba core,

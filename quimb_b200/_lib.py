@@ -105,6 +105,8 @@ def load(build_if_missing=True):
     for name, res, args in (
         ("qb_qr_stab", ci, [ci, i64, i64, vp, vp, vp, ci, vp, ctypes.c_size_t, vp]),
         ("qb_qr_workspace", i64, [ci, i64, i64]),
+        ("qb_qr_route", ci, [i64, i64, P(i64)]),
+        ("qb_svd_route", ci, [i64, i64, ci, P(i64)]),
         ("qb_svd", ci, [ci, i64, i64, vp, vp, vp, vp, vp, ctypes.c_size_t,
                         P(ci), vp]),
         ("qb_svd_workspace", i64, [ci, i64, i64]),

@@ -216,15 +216,43 @@ __global__ void __cluster_dims__(QR_CLUSTER, 1, 1) __launch_bounds__(QR_THREADS,
   }
 }
 
-// R = upper triangle of the factored matrix (first n rows), zeros below
+// R = upper triangle of the factored matrix (first n rows), zeros below,
+// scaled back by 2^e (e from the input's max|x|, 0 when not scaled)
 __global__ void extract_r_kernel(const double *__restrict__ F, int64_t ldf,
-                                 int k, int n, double *__restrict__ R) {
+                                 int k, int n, double *__restrict__ R,
+                                 const unsigned long long *__restrict__ maxbits) {
+  const int e = maxbits ? decomp_scale_exp(*maxbits) : 0;
   int64_t total = (int64_t)k * n;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (int64_t)gridDim.x * blockDim.x) {
     int r = (int)(i / n), c = (int)(i - (int64_t)r * n);
-    R[i] = (c >= r) ? F[(int64_t)r * ldf + c] : 0.0;
+    const double v = (c >= r) ? F[(int64_t)r * ldf + c] : 0.0;
+    R[i] = e ? ldexp(v, e) : v;
   }
+}
+
+// *out = max(*out, bits of max|X|): the bits of non-negative doubles order
+// as unsigned integers, and |NaN| sorts above +inf
+__global__ void __launch_bounds__(256)
+    maxabs_bits_kernel(const double *__restrict__ X, int64_t total,
+                       unsigned long long *__restrict__ out) {
+  unsigned long long mx = 0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (int64_t)gridDim.x * blockDim.x)
+    mx = max(mx, (unsigned long long)__double_as_longlong(fabs(X[i])));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if ((threadIdx.x & 31) == 0 && mx) atomicMax(out, mx);
+}
+
+// F = 2^-e X (a plain copy when e = 0)
+__global__ void __launch_bounds__(256)
+    scale_copy_kernel(const double *__restrict__ X, int64_t total, double *__restrict__ F,
+                      const unsigned long long *__restrict__ maxbits) {
+  const int e = decomp_scale_exp(*maxbits);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (int64_t)gridDim.x * blockDim.x)
+    F[i] = e ? ldexp(X[i], -e) : X[i];
 }
 
 __global__ void set_identity_kernel(double *Q, int64_t m, int64_t n) {
@@ -274,16 +302,60 @@ struct QrGeom {
   int64_t f_off, v_off, t_off, to_off, g_off, w_off, w2_off, sk_off, sk_elems, total;  // doubles
 };
 
+// inner panel width: one row per thread up to 2048 rows, (NB, rows/thread) =
+// (32,1) or (32,2) up to 4096 rows, (16,4) up to 8192, (8,8) up to 16384
+static int qr_inner_width(int64_t m) {
+  if (m <= 4096) return 32;
+  if (m <= 8192) return 16;
+  if (m <= 16384) return 8;
+  return 0;
+}
+
+// panel instantiation for a panel of `rows` rows: 0 (32,1), 1 (32,2),
+// 2 (16,4), 3 (8,8)
+static int qr_panel_kind(int nb, int64_t rows) {
+  if (nb == 32) return rows <= 2048 ? 0 : 1;
+  return nb == 16 ? 2 : 3;
+}
+
+// Aggregation pays when the trailing matrix does not stay in L2; for an
+// L2-resident matrix the extra Gram GEMM + triangular inverse per outer
+// panel cost more than the narrower updates save, so there every inner
+// panel is its own outer panel and its T is used as it comes.  Measured on
+// an H100 SXM at a 400 W power limit, Q and R, without / with aggregation:
+// 2048 x 1024 (16 MiB) 9.3 / 11.2 ms, 2048^2 (32 MiB) 19.7 / 22.7 ms,
+// 3072 x 2048 (48 MiB) 25.5 / 27.1 ms, 4096 x 2048 (64 MiB) 31.2 / 31.4 ms,
+// 4096^2 (128 MiB) 66.3 / 60.3 ms.
+static int qr_outer_width(int64_t m, int64_t n, int nb) {
+  return (m > 4096 || m * n * 8 > (int64_t)48 << 20) ? QR_NBO : nb;
+}
+
+bool qr_route(int64_t m, int64_t n, QrRoute &r) {
+  r = QrRoute{0, 0, 0, 0, 0, 0};
+  r.nb = qr_inner_width(m);
+  if (!r.nb || m <= 0 || n <= 0) return false;
+  const int64_t k = std::min(m, n);
+  r.nbo = qr_outer_width(m, n, r.nb);
+  for (int64_t j0 = 0; j0 < k; j0 += r.nbo) {
+    const int64_t w = std::min<int64_t>(r.nbo, k - j0);
+    ++r.nout;
+    if (w > r.nb) r.wy_t = 1;
+    for (int64_t ji = 0; ji < w; ji += r.nb) {
+      ++r.npan;
+      r.panel_mask |= 1 << qr_panel_kind(r.nb, m - (j0 + ji));
+    }
+  }
+  return true;
+}
+
 static bool qr_geometry(int64_t m, int64_t n, QrGeom &g) {
   const int64_t k = std::min(m, n);
-  if (m <= 4096) g.nb = 32;        // (NB, rows/thread) = (32,1) or (32,2)
-  else if (m <= 8192) g.nb = 16;   // (16,4)
-  else if (m <= 16384) g.nb = 8;   // (8,8)
-  else return false;
+  g.nb = qr_inner_width(m);
+  if (!g.nb) return false;
   const int64_t npan = (k + g.nb - 1) / g.nb;
   const int64_t nout = (k + QR_NBO - 1) / QR_NBO;
   auto al = [](int64_t x) { return (x + 31) / 32 * 32; };  // 256-byte sections
-  int64_t off = 0;
+  int64_t off = 32;                                // [0]: bits of max|X| (qr_maxbits)
   g.f_off = off; off += al(m * n);                 // factored copy of X
   g.v_off = off; off += al(m * (nout * QR_NBO));   // explicit V, one m x w slab per outer panel
   g.t_off = off; off += al(npan * g.nb * g.nb);    // T per inner panel (tau on the diagonal)
@@ -336,9 +408,10 @@ __global__ void __launch_bounds__(QR_NBO)
 }
 
 // Householder QR of row-major X (m x n) -> factored F (in workspace), V, T.
-// Q (m x k) and/or R (k x n) formed on request.  k = min(m, n).
+// Q (m x k) and/or R (k x n) formed on request.  k = min(m, n).  X is
+// factored as 2^-e X (decomp_scale_exp); R is scaled back unless keep_scaled.
 int qr_f64(int64_t m, int64_t n, const double *X, double *Q, double *R,
-           int stabilized, double *ws, cudaStream_t st) {
+           int stabilized, double *ws, cudaStream_t st, bool keep_scaled) {
   QrGeom g;
   if (!qr_geometry(m, n, g)) {
     set_error("qb_qr_stab: m = %lld exceeds the register-panel limit 16384",
@@ -358,19 +431,17 @@ int qr_f64(int64_t m, int64_t n, const double *X, double *Q, double *R,
                                        QR_NBO * (QR_NBO + 1) * 8));
     attr_set = true;
   }
-  QB_CUDA_CHECK(cudaMemcpyAsync(F, X, sizeof(double) * m * n,
-                                cudaMemcpyDeviceToDevice, st));
+  const int blocks = sm_count() * 4;
+  // F = 2^-e X: one max|X| pass decides e on the device (no host round trip)
+  unsigned long long *maxbits = qr_maxbits(ws);
+  QB_CUDA_CHECK(cudaMemsetAsync(maxbits, 0, sizeof(*maxbits), st));
+  maxabs_bits_kernel<<<blocks, 256, 0, st>>>(X, m * n, maxbits);
+  QB_LAUNCH_CHECK();
+  scale_copy_kernel<<<blocks, 256, 0, st>>>(X, m * n, F, maxbits);
+  QB_LAUNCH_CHECK();
   int rc;
   int64_t po = 0;
-  // Aggregation pays when the trailing matrix does not stay in L2; for an
-  // L2-resident matrix the extra Gram GEMM + triangular inverse per outer
-  // panel cost more than the narrower updates save, so there every inner
-  // panel is its own outer panel and its T is used as it comes.  Measured on
-  // an H100 SXM at a 400 W power limit, Q and R, without / with aggregation:
-  // 2048 x 1024 (16 MiB) 9.3 / 11.2 ms, 2048^2 (32 MiB) 19.7 / 22.7 ms,
-  // 3072 x 2048 (48 MiB) 25.5 / 27.1 ms, 4096 x 2048 (64 MiB) 31.2 / 31.4 ms,
-  // 4096^2 (128 MiB) 66.3 / 60.3 ms.
-  const int64_t nbo = (m > 4096 || m * n * 8 > (int64_t)48 << 20) ? QR_NBO : nb;
+  const int64_t nbo = qr_outer_width(m, n, nb);
   for (int64_t j0 = 0; j0 < k; j0 += nbo, ++po) {
     const int w = (int)std::min<int64_t>(nbo, k - j0);   // outer panel width
     const int64_t mp = m - j0;
@@ -385,10 +456,12 @@ int qr_f64(int64_t m, int64_t n, const double *X, double *Q, double *R,
       double *Fp = F + col * n + col;
       double *Vp = Vo + (int64_t)ji * w + ji;   // rows from `col`, columns ji.., ld w
       double *Tp = Ti + (int64_t)(ji / nb) * nb * nb;
-      if (nb == 32 && mpi <= 2048) rc = launch_panel<32, 1>(Fp, n, mpi, nbw, Vp, w, Tp, st);
-      else if (nb == 32) rc = launch_panel<32, 2>(Fp, n, mpi, nbw, Vp, w, Tp, st);
-      else if (nb == 16) rc = launch_panel<16, 4>(Fp, n, mpi, nbw, Vp, w, Tp, st);
-      else rc = launch_panel<8, 8>(Fp, n, mpi, nbw, Vp, w, Tp, st);
+      switch (qr_panel_kind(nb, mpi)) {
+        case 0: rc = launch_panel<32, 1>(Fp, n, mpi, nbw, Vp, w, Tp, st); break;
+        case 1: rc = launch_panel<32, 2>(Fp, n, mpi, nbw, Vp, w, Tp, st); break;
+        case 2: rc = launch_panel<16, 4>(Fp, n, mpi, nbw, Vp, w, Tp, st); break;
+        default: rc = launch_panel<8, 8>(Fp, n, mpi, nbw, Vp, w, Tp, st); break;
+      }
       if (rc) return rc;
       const int64_t nti = w - (ji + nbw);   // rest of the OUTER panel only
       if (nti > 0) {
@@ -419,9 +492,9 @@ int qr_f64(int64_t m, int64_t n, const double *X, double *Q, double *R,
       if ((rc = gemm_f64(Vo, w, 1, W2, nt, 1, C, n, 1, mp, nt, w, -1.0, 1.0, st))) return rc;
     }
   }
-  const int blocks = sm_count() * 4;
   if (R) {
-    extract_r_kernel<<<blocks, 256, 0, st>>>(F, n, (int)k, (int)n, R);
+    extract_r_kernel<<<blocks, 256, 0, st>>>(F, n, (int)k, (int)n, R,
+                                             keep_scaled ? nullptr : maxbits);
     QB_LAUNCH_CHECK();
   }
   if (Q) {
@@ -465,6 +538,17 @@ int64_t qb_qr_workspace(int dtype, int64_t m, int64_t n) {
   QrGeom g;
   if (!qr_geometry(m, n, g)) return -2;
   return g.total * 8;
+}
+
+int qb_qr_route(int64_t m, int64_t n, int64_t *out) {
+  QrRoute r;
+  if (!qr_route(m, n, r)) {
+    set_error("qb_qr_route: unsupported shape %lld x %lld", (long long)m, (long long)n);
+    return -2;
+  }
+  out[0] = r.nb; out[1] = r.nbo; out[2] = r.nout; out[3] = r.panel_mask;
+  out[4] = r.wy_t; out[5] = r.npan;
+  return 0;
 }
 
 int qb_qr_stab(int dtype, int64_t m, int64_t n, const void *X, void *Q,

@@ -39,9 +39,6 @@ namespace qb {
 int svd_tall_f64_v1(int64_t m, int64_t n, const double *X, double *U, double *S,
                     double *VH, double *ws, int *sweeps_out, cudaStream_t st);
 int64_t svd_v1_workspace_doubles(int64_t m, int64_t n);
-int qr_f64(int64_t m, int64_t n, const double *X, double *Q, double *R,
-           int stabilized, double *ws, cudaStream_t st);
-int64_t qr_workspace_doubles(int64_t m, int64_t n);
 
 namespace jac2 {
 
@@ -56,6 +53,7 @@ struct Params {
   int rows_w, rows_v;
   const int2 *pairs;  // column-block pairs of this launch (one per cluster)
   double tol;
+  const double *negl;  // Gram diagonals <= *negl: numerically zero columns
   int *flag;                     // set to 1 when any pair still needed rotating
   unsigned long long *offmax;    // max scaled off-diagonal met (double bits)
   int inner_max;
@@ -73,6 +71,34 @@ __device__ __forceinline__ unsigned long long now_ns() {
     if (P.trace && blockIdx.x == 0 && threadIdx.x == 0)                    \
       P.trace[(size_t)P.trace_slot * 8 + (ph)] = now_ns();              \
   } while (0)
+
+// Which pairs rotate, and which flag a sweep as unconverged.  Both tests are
+// relative to the column norms, so a pair is flagged only if it is rotated:
+//  * a column whose squared norm is at most negl (eps |W|_F, squared) is
+//    numerically zero (rank deficiency).  Rotating it against others only
+//    re-creates rounding noise at the scale of the large column, which never
+//    converges; it takes no part, and its singular value is returned as 0;
+//  * otherwise the measure is |g_pq| / sqrt(g_pp g_qq), formed without
+//    underflow when g_pp g_qq underflows (columns far below the largest);
+//  * a pair rotates when |g_pq| > 1e-300 or its measure exceeds 2^-60 (far
+//    below the convergence tolerance), so small columns that are far from
+//    orthogonal still rotate.
+constexpr double kJacSkip = 1e-300;
+constexpr double kJacRelSkip = 0x1p-60;
+
+__device__ __forceinline__ double pair_off(double v, double gpp, double gqq, double negl) {
+  v = fabs(v);
+  if (!(v > 0.0) || gpp <= negl || gqq <= negl) return 0.0;
+  const double d = gpp * gqq;
+  if (d > 0.0) return v * rsqrt(d);
+  return v / (sqrt(gpp) * sqrt(gqq));
+}
+
+__device__ __forceinline__ bool pair_rotates(double apq, double app, double aqq, double negl) {
+  if (app <= negl || aqq <= negl) return false;
+  const double v = fabs(apq);
+  return v > kJacSkip || (v > 0.0 && v > kJacRelSkip * (sqrt(app) * sqrt(aqq)));
+}
 
 __device__ __forceinline__ void rr_pair(int k, int round, int nblk, int &p, int &q) {
   const int m = nblk - 1;
@@ -207,6 +233,7 @@ __global__ void __launch_bounds__(256, MINB) jacobi_round_kernel(const Params P)
   // warps are descheduled), so co-resident CTAs of other streams get the SM.
   if (rank == 0) {
     double(*G)[JP + 1] = S.Gs;
+    const double negl = *P.negl;
     // full Gram = sum over the cluster in rank order, then symmetrised
     for (int idx = tid; idx < JP * JP; idx += 256) {
       double sum = 0.0;
@@ -222,12 +249,7 @@ __global__ void __launch_bounds__(256, MINB) jacobi_round_kernel(const Params P)
     double mx = 0.0;
     for (int idx = tid; idx < JP * JP; idx += 256) {
       const int r = idx / JP, c = idx % JP;
-      if (r < c) {
-        const double d = G[r][r] * G[c][c];
-        const double v = fabs(G[r][c]);
-        if (d > 0.0) mx = fmax(mx, v * rsqrt(d));
-        else if (v > 0.0) mx = fmax(mx, 1.0);
-      }
+      if (r < c) mx = fmax(mx, pair_off(G[r][c], G[r][r], G[c][c], negl));
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
@@ -272,12 +294,9 @@ __global__ void __launch_bounds__(256, MINB) jacobi_round_kernel(const Params P)
           if (k1 == k2) { S.dg[k1] = gAA; S.dg[16 + k1] = gBB; }
           __syncthreads();
           const double dA1 = S.dg[k1], dB1 = S.dg[16 + k1], dA2 = S.dg[k2], dB2 = S.dg[16 + k2];
-          auto rel = [](double v, double d) {
-            v = fabs(v);
-            return d > 0.0 ? v * rsqrt(d) : (v > 0.0 ? 1.0 : 0.0);
-          };
-          double m = fmax(rel(gAB, dA1 * dB2), rel(gBA, dB1 * dA2));
-          if (k1 != k2) m = fmax(m, fmax(rel(gAA, dA1 * dA2), rel(gBB, dB1 * dB2)));
+          double m = fmax(pair_off(gAB, dA1, dB2, negl), pair_off(gBA, dB1, dA2, negl));
+          if (k1 != k2)
+            m = fmax(m, fmax(pair_off(gAA, dA1, dA2, negl), pair_off(gBB, dB1, dB2, negl)));
 #pragma unroll
           for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
           if (lane == 0) S.redmax[warp] = m;
@@ -296,7 +315,7 @@ __global__ void __launch_bounds__(256, MINB) jacobi_round_kernel(const Params P)
           if (lane < 16) {
             const double app = Gc.A[lane][lane], aqq = Gc.B[16 + lane][lane];
             const double apq = Gc.B[lane][lane];
-            if (fabs(apq) > 1e-300) {
+            if (pair_rotates(apq, app, aqq, negl)) {
               // tan 2t = b / a with a = aqq - app, b = 2 apq, |t| <= pi / 4
               const double a = __dsub_rn(aqq, app), b = __dmul_rn(2.0, apq);
               const double n2 = __fma_rn(a, a, __dmul_rn(b, b));
@@ -607,6 +626,25 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// *negl = (eps |W|_F)^2 from the column norms s (fixed summation order):
+// columns whose squared norm is at most this are numerically zero
+__global__ void __launch_bounds__(256)
+    negligible_kernel(const double *__restrict__ s, int n, double *__restrict__ negl) {
+  __shared__ double sh[256];
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < n; i += 256) acc += s[i] * s[i];
+  sh[threadIdx.x] = acc;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) sh[threadIdx.x] += sh[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const double t = 2.220446049250313e-16;
+    *negl = t * t * sh[0];
+  }
+}
+
 // UR[:, k] = Z[:, perm[k]] * ls[k]   (rows_w x nk, row-major, ld nk), and
 // VH[k, :] = (W[:, perm[k]] / s[perm[k]]) * rs[k]   (nk x rows_w): the kept
 // columns only, with the absorbed powers of the singular values folded in.
@@ -757,10 +795,22 @@ static SideStreams &side_streams() {
   return S;
 }
 
+// Sweeps 1 .. kGraphSweeps - 1 of a multi-group schedule replay a cached CUDA
+// graph (QB_JAC_GRAPH=0: direct launches); later sweeps run direct launches
+// with fuller inner solves (inner_max >= 4).
+constexpr int kGraphSweeps = 25;
+static bool sweep_graph_eligible(int ngroups) {
+  static const bool use_graph = [] {
+    const char *e = getenv("QB_JAC_GRAPH");
+    return !(e && atoi(e) == 0);
+  }();
+  return use_graph && !trace_buffer() && ngroups > 1;
+}
+
 // Jacobi iteration on W (n x npad, ld npad) accumulating rotations in Z
 // (npad x npad).  Returns the number of sweeps (negative: error code).
 static int jacobi_iterate(double *W, double *Z, int64_t n, int64_t npad, int2 *d_pairs,
-                          int *flag, int *sweeps_out, cudaStream_t st) {
+                          int *flag, const double *negl, int *sweeps_out, cudaStream_t st) {
   const int nblk = (int)(npad / JB);
   const Config cfg = pick_config(nblk);
   Schedule sched;
@@ -770,6 +820,7 @@ static int jacobi_iterate(double *W, double *Z, int64_t n, int64_t npad, int2 *d
   Params P;
   P.W = W; P.V = Z; P.ld = npad; P.rows_w = (int)n; P.rows_v = Z ? (int)npad : 0;
   P.tol = 1e-15 * sqrt((double)n) * 8.0;
+  P.negl = negl;
   P.flag = flag;
   P.offmax = reinterpret_cast<unsigned long long *>(flag + 2);
   P.trace = trace_buffer() ? trace_buffer() + 16 * 8192 : nullptr;
@@ -829,11 +880,7 @@ static int jacobi_iterate(double *W, double *Z, int64_t n, int64_t npad, int2 *d
     long stagger = 0;
   };
   static thread_local SweepGraph SG;
-  static const bool use_graph = [] {
-    const char *e = getenv("QB_JAC_GRAPH");
-    return !(e && atoi(e) == 0);
-  }();
-  const bool graph_ok = use_graph && !P.trace && multi;
+  const bool graph_ok = sweep_graph_eligible(sched.ngroups);
   auto graph_matches = [&]() {
     return SG.exec && SG.W == W && SG.Z == Z && SG.pairs == d_pairs && SG.n == n &&
            SG.npad == npad && SG.cfg.cs == cfg.cs && SG.cfg.ch == cfg.ch &&
@@ -842,10 +889,10 @@ static int jacobi_iterate(double *W, double *Z, int64_t n, int64_t npad, int2 *d
   };
   for (; sweeps < max_sweeps && !done; ++sweeps) {
     const double t0 = wall();
-    P.inner_max = (sweeps < 25) ? inner0 : std::max(inner0, 4);
+    P.inner_max = (sweeps < kGraphSweeps) ? inner0 : std::max(inner0, 4);
     QB_CUDA_CHECK(cudaMemsetAsync(flag, 0, 16, st));
     bool launched = false;
-    if (graph_ok && sweeps >= 1 && sweeps < 25) {
+    if (graph_ok && sweeps >= 1 && sweeps < kGraphSweeps) {
       if (!graph_matches()) {
         if (SG.exec) { cudaGraphExecDestroy(SG.exec); SG.exec = nullptr; }
         cudaGraph_t gr = nullptr;
@@ -919,6 +966,22 @@ static bool absorb_plan(int absorb, AbsorbPlan &a) {
   return false;
 }
 
+// Epilogue algorithm of an absorb mode (see svd_trunc_tall)
+enum { EPI_ACCUMULATE = 0, EPI_LEFT = 1, EPI_RIGHT = 2, EPI_VALUES = 3 };
+static int epilogue_kind(int absorb) {
+  static const bool no_accum_ok = [] {
+    const char *e = getenv("QB_SVD_ACCUMULATE");
+    return !(e && atoi(e) == 1);
+  }();
+  if (!no_accum_ok) return EPI_ACCUMULATE;
+  if (absorb == QB_ABSORB_LEFT || absorb == QB_ABSORB_LFACTOR || absorb == QB_ABSORB_RORTHOG)
+    return EPI_LEFT;
+  if (absorb == QB_ABSORB_RIGHT || absorb == QB_ABSORB_LORTHOG || absorb == QB_ABSORB_RFACTOR)
+    return EPI_RIGHT;
+  if (absorb == QB_ABSORB_S) return EPI_VALUES;
+  return EPI_ACCUMULATE;
+}
+
 // SVD of row-major X (m x n), m >= n, with the truncation / absorb epilogue.
 // U: m x nk (ld nk), S: nk, VH: nk x n, written compactly for the kept rank.
 static int svd_trunc_tall(int64_t m, int64_t n, const double *X, double cutoff,
@@ -953,22 +1016,29 @@ static int svd_trunc_tall(int64_t m, int64_t n, const double *X, double cutoff,
   // transpose in the host layer for square input.)  Modes that return BOTH
   // isometries (None, both, lsqrt, rsqrt) keep the accumulation: dividing the
   // other factor by tiny singular values would lose its orthogonality.
-  const bool left_family = absorb == QB_ABSORB_LEFT || absorb == QB_ABSORB_LFACTOR ||
-                           absorb == QB_ABSORB_RORTHOG;
-  // mirror family (U the isometry): rotate the columns of R itself, R Z' = U_R S,
-  // so U = Q1 U_R from the normalised columns and (f S) V^T = f U_R^T R by one GEMM
-  const bool right_family = absorb == QB_ABSORB_RIGHT || absorb == QB_ABSORB_LORTHOG ||
-                            absorb == QB_ABSORB_RFACTOR;
-  const bool vals_only = absorb == QB_ABSORB_S;
-  static const bool no_accum_ok = [] {
-    const char *e = getenv("QB_SVD_ACCUMULATE");
-    return !(e && atoi(e) == 1);
-  }();
-  const bool accumulate = !((left_family || right_family || vals_only) && no_accum_ok);
+  // (Mirror family, U the isometry: rotate the columns of R itself,
+  // R Z' = U_R S, so U = Q1 U_R from the normalised columns and
+  // (f S) V^T = f U_R^T R by one GEMM.)
+  const int epi = epilogue_kind(absorb);
+  const bool right_family = epi == EPI_RIGHT;
+  const bool vals_only = epi == EPI_VALUES;
+  const bool accumulate = epi == EPI_ACCUMULATE;
   const bool need_u = ap.want_l && U;
+  // R in the units of 2^-e X (decomp_scale_exp): the Jacobi iteration, the
+  // rotated columns and their norms stay scaled, the singular values the keep
+  // rule and the absorbed powers see are scaled back
   int rc = qr_f64(m, n, X, (need_u && (accumulate || right_family)) ? Q1 : nullptr, R,
-                  /*stabilized=*/0, ws + g.qr_off, st);
+                  /*stabilized=*/0, ws + g.qr_off, st, /*keep_scaled=*/true);
   if (rc) return rc;
+  unsigned long long maxbits = 0;
+  QB_CUDA_CHECK(cudaMemcpyAsync(&maxbits, qr_maxbits(ws + g.qr_off), sizeof(maxbits),
+                                cudaMemcpyDeviceToHost, st));
+  QB_CUDA_CHECK(cudaStreamSynchronize(st));
+  if (!decomp_finite(maxbits)) {
+    set_error("qb_svd: the input contains NaN or Inf");
+    return -9;
+  }
+  const int e = decomp_scale_exp(maxbits);
   const int64_t npad = g.npad;
   // W = R^T, or R itself for the accumulation-free right family
   pad_copy_kernel<<<blocks, 256, 0, st>>>(R, n, n, n, W, npad, n,
@@ -980,14 +1050,28 @@ static int svd_trunc_tall(int64_t m, int64_t n, const double *X, double cutoff,
   } else {
     Z = nullptr;
   }
-  int sw = jacobi_iterate(W, Z, n, npad, d_pairs, flag, sweeps_out, st);
+  double *negl = reinterpret_cast<double *>(flag) + 4;
+  colnorm_kernel<<<(unsigned)(npad / 32), 256, 0, st>>>(W, npad, (int)n, (int)npad, sv);
+  QB_LAUNCH_CHECK();
+  negligible_kernel<<<1, 256, 0, st>>>(sv, (int)n, negl);
+  QB_LAUNCH_CHECK();
+  int sw = jacobi_iterate(W, Z, n, npad, d_pairs, flag, negl, sweeps_out, st);
   if (sw < 0) return -sw;
   colnorm_kernel<<<(unsigned)(npad / 32), 256, 0, st>>>(W, npad, (int)n, (int)npad, sv);
   QB_LAUNCH_CHECK();
   std::vector<double> hs(npad);
+  double hnegl = 0.0;
   QB_CUDA_CHECK(cudaMemcpyAsync(hs.data(), sv, sizeof(double) * npad,
                                 cudaMemcpyDeviceToHost, st));
+  QB_CUDA_CHECK(cudaMemcpyAsync(&hnegl, negl, sizeof(double), cudaMemcpyDeviceToHost, st));
   QB_CUDA_CHECK(cudaStreamSynchronize(st));
+  // numerically zero columns (they took no part in the iteration): singular
+  // value 0, so the caller completes their vectors to isometries
+  bool zeroed = false;
+  for (int64_t i = 0; i < n; ++i)
+    if (hs[i] > 0.0 && hs[i] * hs[i] <= hnegl) { hs[i] = 0.0; zeroed = true; }
+  if (zeroed)
+    QB_CUDA_CHECK(cudaMemcpyAsync(sv, hs.data(), sizeof(double) * n, cudaMemcpyHostToDevice, st));
   std::vector<int> hp(npad);
   for (int i = 0; i < npad; ++i) hp[i] = i;
   std::stable_sort(hp.begin(), hp.end(), [&](int a, int b) {
@@ -995,8 +1079,12 @@ static int svd_trunc_tall(int64_t m, int64_t n, const double *X, double cutoff,
     if (pa != pb) return pb;
     return hs[a] > hs[b];
   });
-  std::vector<double> ss(n);
-  for (int i = 0; i < n; ++i) ss[i] = hs[hp[i]];
+  // sorted singular values: ss in the caller's units, ssc in those of 2^-e X
+  std::vector<double> ss(n), ssc(n);
+  for (int i = 0; i < n; ++i) {
+    ssc[i] = hs[hp[i]];
+    ss[i] = e ? ldexp(ssc[i], e) : ssc[i];
+  }
   // ---- the reference's keep rule / renormalisation on the sorted values ----
   int64_t nk = n;
   double f = 1.0, err = 0.0;
@@ -1030,9 +1118,10 @@ static int svd_trunc_tall(int64_t m, int64_t n, const double *X, double cutoff,
     }
     if (right_family) {
       // U_R (n x nk) = normalised rotated columns of R (scale 1 / s, null
-      // columns stay zero); U = Q1 U_R; (f S) V^T = f U_R^T R
+      // columns stay zero); U = Q1 U_R; (f S) V^T = f U_R^T R (R scaled by
+      // 2^-e, so the GEMM takes f 2^e)
       std::vector<double> inv(nk);
-      for (int64_t i = 0; i < nk; ++i) inv[i] = ss[i] > 0.0 ? 1.0 / ss[i] : 0.0;
+      for (int64_t i = 0; i < nk; ++i) inv[i] = ssc[i] > 0.0 ? 1.0 / ssc[i] : 0.0;
       QB_CUDA_CHECK(cudaMemcpyAsync(d_scale, inv.data(), sizeof(double) * nk,
                                     cudaMemcpyHostToDevice, st));
       gather_scaled_kernel<<<blocks, 256, 0, st>>>(W, W, npad, (int)n, (int)nk, perm, sv,
@@ -1044,7 +1133,7 @@ static int svd_trunc_tall(int64_t m, int64_t n, const double *X, double cutoff,
         if (rc) return rc;
       }
       if (need_v) {
-        rc = gemm_f64(UR, 1, nk, R, n, 1, VH, n, 1, nk, n, n, f, 0.0, st);
+        rc = gemm_f64(UR, 1, nk, R, n, 1, VH, n, 1, nk, n, n, e ? ldexp(f, e) : f, 0.0, st);
         if (rc) return rc;
       }
       return 0;
@@ -1158,6 +1247,34 @@ int64_t qb_debug_jacobi_schedule(int nblk, int groups, int32_t *out, int64_t cap
         }
       }
   return n;
+}
+
+// Host only: what qb_svd_trunc (qb_svd: absorb = QB_ABSORB_FULL) launches for
+// a tall m x n matrix (m >= n), from the decisions of the launch path.
+int qb_svd_route(int64_t m, int64_t n, int absorb, int64_t *out) {
+  jac2::Geom g;
+  QrRoute q;
+  AbsorbPlan ap;
+  if (m < n || n <= 0 || !jac2::geometry(m, n, g) || !qr_route(m, n, q)) {
+    set_error("qb_svd_route: unsupported shape %lld x %lld", (long long)m, (long long)n);
+    return -2;
+  }
+  if (!absorb_plan(absorb, ap)) {
+    set_error("qb_svd_route: invalid absorb code %d", absorb);
+    return -8;
+  }
+  const int nblk = (int)(g.npad / jac2::JB);
+  const jac2::Config c = jac2::pick_config(nblk);
+  jac2::Schedule S;
+  jac2::build_schedule(nblk, c.groups, S);
+  int64_t rounds = 0;
+  for (const auto &ph : S.phases)
+    for (const auto &gr : ph.rounds) rounds += (int64_t)gr.size();
+  out[0] = g.npad; out[1] = nblk; out[2] = S.ngroups; out[3] = c.cs; out[4] = c.ch;
+  out[5] = c.stg; out[6] = epilogue_kind(absorb);
+  out[7] = jac2::sweep_graph_eligible(S.ngroups) ? jac2::kGraphSweeps - 1 : 0;
+  out[8] = q.panel_mask; out[9] = q.wy_t; out[10] = rounds;
+  return 0;
 }
 
 int qb_svd_trunc(int dtype, int64_t m, int64_t n, const void *X, double cutoff,

@@ -19,6 +19,7 @@ kernels through the interleaved real embedding
 
 import ctypes
 import functools
+import math
 
 import numpy as np
 import torch
@@ -121,9 +122,10 @@ def qr(x, stabilized=False, want_q=True, want_r=True):
         return Q, R
     lib = _lib.load()
     dev = x.t.device
-    if m > _QR_MAX_ROWS and m >= n:
+    path = _qr_path(m, n)
+    if path == "tsqr":
         return _tsqr(x, stabilized, want_q, want_r)
-    if m < n:
+    if path == "wide":
         # QR of the leading m x m block, R2 = Q^T X[:, m:]
         q, r1 = qr(Array(x.t[:, :m]), stabilized=stabilized)
         r2 = ops.tensordot(q, Array(x.t[:, m:]), axes=((0,), (0,)))
@@ -149,17 +151,34 @@ def qr(x, stabilized=False, want_q=True, want_r=True):
 _QR_MAX_ROWS = 16384
 
 
+def _qr_path(m, n):
+    """Host-layer decision of :func:`qr` for a real m x n matrix: ``"tsqr"``
+    (more than ``_QR_MAX_ROWS`` rows: row blocks), ``"wide"`` (m < n: QR of
+    the leading m x m block) or ``"kernel"`` (one ``qb_qr_stab`` call)."""
+    if m > _QR_MAX_ROWS and m >= n:
+        return "tsqr"
+    if m < n:
+        return "wide"
+    return "kernel"
+
+
+def _tsqr_blocks(m, n):
+    """(row blocks, rows per block) of the TSQR of an m x n matrix."""
+    nblk = -(-m // _QR_MAX_ROWS)
+    rows = -(-m // nblk)
+    if rows < n or nblk * n >= m:
+        raise ValueError(f"quimb_b200.linalg.qr: shape {(m, n)} is not supported "
+                         f"(more than {_QR_MAX_ROWS} rows and {n} columns)")
+    return nblk, rows
+
+
 def _tsqr(x, stabilized, want_q, want_r):
     """Tall-skinny QR for m > 16384 rows (e.g. the (chi d D^2) x (chi D)
     boundary tensors of BASELINE config 5): row blocks are factored
     independently, the stacked R factors are factored again (recursively), and
     Q is assembled with one tensor-core GEMM per block."""
     m, n = x.shape
-    nblk = -(-m // _QR_MAX_ROWS)
-    rows = -(-m // nblk)
-    if rows < n or nblk * n >= m:
-        raise ValueError(f"quimb_b200.linalg.qr: shape {x.shape} is not supported "
-                         f"(more than {_QR_MAX_ROWS} rows and {n} columns)")
+    nblk, rows = _tsqr_blocks(m, n)
     qs, rs = [], []
     for lo in range(0, m, rows):
         q, r = qr(Array(x.t[lo:lo + rows]), stabilized=False, want_q=want_q)
@@ -301,13 +320,14 @@ def svd(x, full_matrices=False, return_sweeps=False):
     m, n = x.shape
     if x.t.dtype == torch.complex128:
         return _svd_complex(x, return_sweeps)
-    if m < n:
+    path = _svd_path(m, n)
+    if path == "transpose":
         xt = ops.materialize(Array(x.t.t()))
         out = svd(xt, return_sweeps=return_sweeps)
         u, s, vh = out[:3]
         res = (Array(vh.t.t()), s, Array(u.t.t()))
         return res + (out[3],) if return_sweeps else res
-    if m > _QR_MAX_ROWS:
+    if path == "qr_first":
         # X = Q R (blocked QR), R = Ur s VH (Jacobi), U = Q Ur (one GEMM)
         q, r = qr(x)
         out = svd(r, return_sweeps=return_sweeps)
@@ -327,6 +347,11 @@ def svd(x, full_matrices=False, return_sweeps=False):
                     S.data_ptr(), VH.data_ptr(), ws.data_ptr(), ws.numel(),
                     ctypes.byref(sweeps), _lib.stream_ptr())
     _lib.check(rc, "qb_svd")
+    # numerically zero columns come back with s = 0 and null rows of VH
+    # (sorted last): complete them, VH is an isometry like LAPACK's
+    nnull = int((S == 0).sum())
+    if nnull:
+        _complete_isometry(VH, list(range(n - nnull, n)), rows=True)
     out = (Array(U), Array(S), Array(VH))
     return out + (sweeps.value,) if return_sweeps else out
 
@@ -336,6 +361,93 @@ _MIRROR_ABSORB = {100: 100, 2: 2, -1: 1, 1: -1, -10: 11, 11: -10, -11: 10, 10: -
 # absorb codes whose right (resp. left) factor is returned as an isometry
 _ISO_RIGHT = (100, -1, -11)
 _ISO_LEFT = (100, 1, 10)
+
+
+def _svd_path(m, n, code=None):
+    """Host-layer decision of :func:`svd` (``code`` None) and
+    :func:`svd_trunc` (quimb's absorb code) for a real m x n matrix:
+    ``"transpose"`` (m < n; for ``svd_trunc`` also square input whose LEFT
+    factor is the isometry, which the kernel serves without accumulated
+    rotations when mirrored), ``"qr_first"`` (more than ``_QR_MAX_ROWS`` rows:
+    blocked QR, then the SVD of R) or ``"kernel"``."""
+    if m < n or (code is not None and m == n and code in (1, 10, 11)):
+        return "transpose"
+    if m > _QR_MAX_ROWS:
+        return "qr_first"
+    return "kernel"
+
+
+def _qr_kernel_route(m, n):
+    out = (ctypes.c_int64 * 16)()
+    _lib.check(_lib.load().qb_qr_route(m, n, out), "qb_qr_route")
+    return {"shape": (m, n), "nb": out[0], "nbo": out[1], "outer_panels": out[2],
+            "panel_mask": out[3], "wy_t": bool(out[4]), "inner_panels": out[5]}
+
+
+def route_qr(shape, dtype=torch.float64):
+    """Which kernels :func:`qr` runs for a matrix of this shape and dtype,
+    from the decisions it takes itself.  ``kernels`` lists the route of every
+    ``qb_qr_stab`` call (``qb_qr_route``: inner / outer panel width, the
+    panel-instantiation bitmask, whether aggregated T factors are formed);
+    ``panel_mask`` / ``wy_t`` are their union.  Complex input runs on its real
+    embedding (and leaves it for the SVD route when the data are
+    ill-conditioned, which no shape decides)."""
+    m, n = (int(s) for s in shape)
+    cplx = torch.empty((), dtype=dtype).is_complex()
+    if cplx:
+        m, n = 2 * m, 2 * n
+    path = _qr_path(m, n)
+    res = {"complex_embed": cplx, "path": path, "wide": path == "wide", "tsqr_blocks": 0}
+    if path == "tsqr":
+        nblk, rows = _tsqr_blocks(m, n)
+        res["tsqr_blocks"] = nblk
+        shapes = sorted({(rows, n), (m - (nblk - 1) * rows, n)})
+        kernels = [_qr_kernel_route(*s) for s in shapes]
+        kernels += route_qr((nblk * n, n))["kernels"]
+    else:
+        kernels = [_qr_kernel_route(m, min(m, n))] if path == "wide" else [_qr_kernel_route(m, n)]
+    res["kernels"] = kernels
+    res["panel_mask"] = functools.reduce(lambda a, k: a | k["panel_mask"], kernels, 0)
+    res["wy_t"] = any(k["wy_t"] for k in kernels)
+    return res
+
+
+_EPILOGUES = ("accumulate", "left", "right", "values")
+
+
+def route_svd(shape, dtype=torch.float64, absorb=None):
+    """Which kernels :func:`svd` (``absorb`` None) or :func:`svd_trunc`
+    (quimb's absorb code) runs for a matrix of this shape and dtype, from the
+    decisions they take themselves: complex embedding, the wide / square
+    mirror transpose, the QR preconditioning above ``_QR_MAX_ROWS`` rows, and
+    ``qb_svd_route`` of the Jacobi kernel call (padded width, column blocks,
+    stream groups, cluster size, chunk rows, stages, epilogue, graph-replayed
+    sweeps, round launches per sweep, its QR preconditioner's panel mask and
+    aggregation)."""
+    m, n = (int(s) for s in shape)
+    cplx = torch.empty((), dtype=dtype).is_complex()
+    if cplx:
+        if absorb is not None:
+            raise TypeError("svd_trunc: float64 only (other dtypes go through svd())")
+        m, n = 2 * m, 2 * n
+    code = None if absorb is None else int(absorb)
+    res = {"complex_embed": cplx, "transpose": False, "mirror": False, "qr_first": None}
+    if _svd_path(m, n, code) == "transpose":
+        res["transpose"] = m < n
+        res["mirror"] = m == n
+        m, n = n, m
+        code = None if code is None else _MIRROR_ABSORB[code]
+    if _svd_path(m, n, code) == "qr_first":
+        res["qr_first"] = route_qr((m, n))
+        m = n
+    out = (ctypes.c_int64 * 16)()
+    kcode = 100 if code is None else code
+    _lib.check(_lib.load().qb_svd_route(m, n, kcode, out), "qb_svd_route")
+    res.update({"kernel_shape": (m, n), "absorb": kcode, "npad": out[0], "nblk": out[1],
+                "groups": out[2], "cluster": out[3], "chunk": out[4], "stages": out[5],
+                "epilogue": _EPILOGUES[out[6]], "graph_sweeps": out[7],
+                "qr_panel_mask": out[8], "qr_wy_t": bool(out[9]), "rounds": out[10]})
+    return res
 
 
 def svd_trunc(x, cutoff=-1.0, cutoff_mode=4, max_bond=-1, absorb=0, renorm=0, info=None):
@@ -351,7 +463,8 @@ def svd_trunc(x, cutoff=-1.0, cutoff_mode=4, max_bond=-1, absorb=0, renorm=0, in
         raise TypeError("svd_trunc: float64 only (other dtypes go through svd())")
     m, n = x.shape
     code = 100 if absorb is None else int(absorb)
-    if m < n or (m == n and code in (1, 10, 11)):
+    path = _svd_path(m, n, code)
+    if path == "transpose":
         # X^T = V s U^T: factor the transpose, swap the roles of the factors.
         # Also taken for SQUARE input whose LEFT factor is to be the isometry
         # ('right' / 'lorthog' / 'rfactor': DMRG's right-moving sweep): the
@@ -365,7 +478,7 @@ def svd_trunc(x, cutoff=-1.0, cutoff_mode=4, max_bond=-1, absorb=0, renorm=0, in
         left = None if r is None else Array(r.t.t())
         right = None if l is None else Array(l.t.t())
         return left, s, right
-    if m > _QR_MAX_ROWS:
+    if path == "qr_first":
         # blocked QR first (m beyond the register-panel limit), then the core
         q, rr = qr(x)
         l, s, r = svd_trunc(rr, cutoff, cutoff_mode, max_bond, code, renorm, info)
@@ -484,7 +597,9 @@ def eigh(x, host_below=None):
     ``w = s - sigma``; eigenvalues are accurate to ``eps * |x|_F`` like any
     backward-stable dense eigensolver.  complex128 goes through the real
     embedding, float32 / complex64 through the exact widening pass (both
-    inherited from :func:`svd`).  ``sigma`` never leaves the device."""
+    inherited from :func:`svd`).  ``sigma`` stays on the device; max|x| is
+    read once on the host to decide the power-of-two scaling (and to reject
+    NaN / Inf) before the SVD, which synchronises anyway."""
     x = ops.asarray(x)
     if x.ndim != 2 or x.shape[0] != x.shape[1]:
         raise ValueError(f"eigh: expected a square matrix, got shape {x.shape}")
@@ -497,13 +612,37 @@ def eigh(x, host_below=None):
         return ops.asarray(w), ops.asarray(v)
     xm = ops.materialize(x, force=True)            # private copy (shifted in place)
     _lib.require_cuda(xm.t)
+    # |x|_F squares the entries: outside [2^-200, 2^200] (the window of the
+    # SVD kernel, csrc/internal.h) x is scaled by 2^-e first, like the SVD
+    # scales its own input, and the eigenvalues are scaled back
+    amax = float(torch.amax(torch.abs(xm.t))) if xm.t.numel() else 0.0
+    if not math.isfinite(amax):
+        raise ValueError("eigh: the input contains NaN or Inf")
+    e = math.frexp(amax)[1] - 1 if amax > 0.0 else 0
+    if abs(e) <= _DECOMP_SAFE_EXP:
+        e = 0
+    for f in _pow2_factors(-e):
+        xm.t.mul_(f)
     sigma = norm(xm)                               # 0-d, real, on the device
     sg = sigma.t.to(_REAL_OF[xm.t.dtype])
     xm.t.diagonal().add_(sg)
     _, s, VH = svd(xm)
     w = (s.t - sg.to(s.t.dtype)).flip(0)           # ascending
+    for f in _pow2_factors(e):
+        w = w * f
     v = Array(VH.t.flip(0).transpose(0, 1), not VH.cj)   # v[:, i] = conj(VH[k-1-i, :])
     return Array(w), v
+
+
+_DECOMP_SAFE_EXP = 200
+
+
+def _pow2_factors(k):
+    """2^k as at most two representable factors (|k| <= 2044)."""
+    if k == 0:
+        return ()
+    h = k // 2
+    return (math.ldexp(1.0, h), math.ldexp(1.0, k - h))
 
 
 _REAL_OF = {torch.float32: torch.float32, torch.float64: torch.float64,

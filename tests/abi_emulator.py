@@ -36,7 +36,7 @@ _REAL = {_lib.QB_F32: np.float32, _lib.QB_F64: np.float64,
 _HOST_ONLY = {
     "qb_abi_version", "qb_last_error", "qb_contract_pair_plan", "qb_contract_pair_route",
     "qb_contract_pair_workspace", "qb_dot_workspace", "qb_multi_dot_workspace",
-    "qb_qr_workspace", "qb_svd_workspace", "qb_svals_to_keep",
+    "qb_qr_workspace", "qb_svd_workspace", "qb_svals_to_keep", "qb_qr_route", "qb_svd_route",
 }
 
 
@@ -340,7 +340,12 @@ class EmulatedLib:
             return self._fail(-8, "qb_qr_stab: workspace too small")
         self._tick("qb_qr_stab")
         x = _flat(X, m * n, np.float64).reshape(m, n)
-        q, r = np.linalg.qr(x)
+        # the kernel factors 2^-e x outside max|x| in [2^-200, 2^200]
+        mx = np.abs(x).max()
+        e = int(np.frexp(mx)[1]) - 1 if np.isfinite(mx) and mx > 0 else 0
+        e = e if abs(e) > 200 else 0
+        q, r = np.linalg.qr(np.ldexp(x, -e))
+        r = np.ldexp(r, e)
         if stabilized:
             sg = np.where(np.diag(r) < 0, -1.0, 1.0)
             q = q * sg[None, :]
@@ -363,8 +368,10 @@ class EmulatedLib:
             return self._fail(-8, "qb_svd: workspace too small")
         if m < n:
             return self._fail(-2, "qb_svd: m < n -- pass the transpose")
-        self._tick("qb_svd")
         x = _flat(X, m * n, np.float64).reshape(m, n)
+        if not np.all(np.isfinite(x)):
+            return self._fail(-9, "qb_svd: the input contains NaN or Inf")
+        self._tick("qb_svd")
         u, s, vh = np.linalg.svd(x, full_matrices=False)
         _flat(U, m * n, np.float64).reshape(m, n)[...] = u
         _flat(S, n, np.float64)[...] = s
@@ -395,8 +402,10 @@ class EmulatedLib:
         if plan is None:
             return self._fail(-8, f"qb_svd_trunc: invalid absorb code {absorb}")
         lpow, rpow, want_l, want_r, want_s = plan
-        self._tick("qb_svd_trunc")
         x = _flat(X, m * n, np.float64).reshape(m, n)
+        if not np.all(np.isfinite(x)):
+            return self._fail(-9, "qb_svd: the input contains NaN or Inf")
+        self._tick("qb_svd_trunc")
         u, s, vh = np.linalg.svd(x, full_matrices=False)
         s = np.where(s > 1e-300 * max(s[0], 1e-300), s, 0.0) if s.size else s
         nk = ctypes.c_int64(0)

@@ -423,3 +423,56 @@ def test_bond_shard_exchange_argument():
     assert s.slab(10) == (0, 10)
     with pytest.raises(ValueError):
         BondShard(rank=0, world_size=1, exchange="mpi")
+
+
+def test_decomposition_routes_pinned_for_benchmark_shapes():
+    """The DMRG split of the benchmark (a 2048 x 2048 svd_trunc, right sweep:
+    absorb 'right' mirrored onto the accumulation-free left family) and the
+    TSQR of the boundary configuration's (chi d D^2) x (chi D) tensors."""
+    from quimb_b200 import linalg
+    r = linalg.route_svd((2048, 2048), absorb=1)
+    assert (r["mirror"], r["transpose"], r["qr_first"], r["absorb"]) == (True, False, None, -1)
+    assert (r["npad"], r["nblk"], r["groups"], r["cluster"], r["chunk"], r["stages"]) == \
+        (2048, 128, 4, 2, 64, 4)
+    assert (r["epilogue"], r["graph_sweeps"], r["qr_panel_mask"], r["qr_wy_t"]) == \
+        ("left", 24, 0b0001, False)
+    assert linalg.route_svd((2048, 2048))["epilogue"] == "accumulate"
+    q = linalg.route_qr((128 * 4 * 64, 128 * 8))          # chi = 128, d = 4, D = 8
+    assert q["path"] == "tsqr" and q["tsqr_blocks"] == 2
+    assert [k["shape"] for k in q["kernels"]] == [(16384, 1024), (2048, 1024)]
+    assert (q["panel_mask"], q["wy_t"]) == (0b1001, True)
+
+
+def test_decomposition_route_search_reaches_every_route():
+    """The GPU decomposition route tests find a grid shape for every route."""
+    from tests import decomp_oracle as do
+    found = do.search_routes()
+    missing = [k for k in do.QR_KEYS + do.SVD_KEYS if k not in found]
+    assert not missing, missing
+    assert found[("svd", "groups", "fallback")][3]["nblk"] == 66
+
+
+def test_decomposition_oracle_is_exact():
+    """The dyadic constructions are exact and orthogonal in integer
+    arithmetic, and the numpy / mpmath references agree with them."""
+    from tests import decomp_oracle as do
+    rng = np.random.default_rng(3)
+    for m, k in ((1, 1), (17, 5), (100, 48), (2049, 33)):
+        X, J = do.isometry(m, k, rng)
+        G = X.astype(object).T.dot(X.astype(object))          # exact integers
+        assert all(G[i, j] == (4 ** J if i == j else 0) for i in range(k) for j in range(k))
+    A, Q0, R0, kappa = do.qr_case(100, 40, rng)
+    assert kappa <= 11 and np.array_equal(Q0 @ R0, A)
+    q, r = np.linalg.qr(A)
+    sg = np.sign(np.diag(r))
+    do.check_qr(A, q * sg, r * sg[:, None], kappa=kappa, Q0=Q0, R0=R0)
+    for kind in ("separated", "clusters", "zeros", "graded", "gap"):
+        A, U0, s, V0 = do.svd_case(60, 40, kind, rng)
+        assert np.array_equal((U0 * s) @ V0.T, A)
+        u, ss, vh = np.linalg.svd(A, full_matrices=False)
+        do.check_svd(A, u, ss, vh, s, U0, V0)
+    pytest.importorskip("mpmath")
+    B = rng.standard_normal((30, 20))
+    np.testing.assert_allclose(do.mp_svd(B), np.linalg.svd(B, compute_uv=False), rtol=1e-13)
+    r = np.linalg.qr(B)[1]
+    np.testing.assert_allclose(do.mp_qr_r(B), r * np.sign(np.diag(r))[:, None], atol=1e-13)
