@@ -94,9 +94,10 @@ enum {
   QB_ENGINE_DMMA = 1, /* native fp64 tensor-core path (DMMA)          */
   QB_ENGINE_OZAKI = 2, /* int8 tensor-core (wgmma) error-free-split path */
   QB_ENGINE_STREAM = 3, /* HBM-bound streaming path for small-operator
-                         * steps (N <= 16 and K <= 16 after mode grouping:
-                         * gate application); other shapes take the DMMA
-                         * path.  Opt-in: not timed on the H100.        */
+                         * steps (after mode grouping N, K <= 32 for f64,
+                         * N, K <= 16 for c128: gate application); other
+                         * shapes take the DMMA path.  Opt-in: not timed
+                         * on the H100.                                 */
   /* OR-able flag: the caller guarantees that bytes [0, 1024) of `workspace`
    * (the stream-K flag words) were zero before its first use and are written
    * by this library only -- which always leaves them zero again -- so the
@@ -169,8 +170,9 @@ int qb_contract_pair_plan(const qb_tensor_t *A, const int32_t *labelsA,
  * out[3] = stream-K grid (CTAs, 0 otherwise), out[4] = stream-K head cost
  * (k-blocks), out[5] = DMMA k-block depth, out[6] = cfg-0 shared-memory
  * layout of real operands (a_kmajor * 2 + b_kmajor; -1: runtime layout),
- * out[7] = SM count the planner used, out[8] = kernels launched (beta = 0).
- * The caller provides 16 slots.
+ * out[7] = SM count the planner used, out[8] = kernels launched (beta = 0),
+ * out[9] / out[10] = compiled (KMAX, NMAX) variant of the streaming engine
+ * (0 for every other route).  The caller provides 16 slots.
  */
 int qb_contract_pair_route(const qb_tensor_t *A, const int32_t *labelsA,
                            const qb_tensor_t *B, const int32_t *labelsB,
@@ -205,7 +207,8 @@ int qb_contract_batched(const qb_tensor_t *A0, const int32_t *labelsA,
 /* dst (any strides) = src (any strides), same shape; optional conjugation */
 int qb_permute(const qb_tensor_t *src, qb_tensor_t *dst, int conj,
                void *stream);
-/* y = alpha * x + beta * y over n contiguous elements (alpha,beta: re,im) */
+/* y = alpha * x + beta * y over n contiguous elements (alpha,beta: re,im);
+ * beta = 0 does not read y, so y may hold NaN / Inf or be uninitialised */
 int qb_axpby(int dtype, int64_t n, const double alpha[2], const void *x,
              const double beta[2], void *y, void *stream);
 /* x *= alpha / (*dev_scalar)  (dev_scalar may be NULL); Lanczos normalise */

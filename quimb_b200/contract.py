@@ -284,7 +284,11 @@ def route_pair(a_shape, a_strides, la, b_shape, b_strides, lb, c_shape,
     count of the current device or the H100 SXM's 132 without one).
 
     ``ptrs`` = (a, b, c) base addresses; the vector loads depend on 16-byte
-    alignment, so pass the real ones when the route of a view matters."""
+    alignment, so pass the real ones when the route of a view matters.
+
+    A streaming-engine route (kind ``"stream"``) also carries ``stream_k`` /
+    ``stream_n``, the compiled (KMAX, NMAX) variant it launches; other routes
+    have no variant and do not carry these keys."""
     lib = _lib.load()
     pa, pb, pc = ptrs if ptrs is not None else (0x10000000,) * 3
     da = _lib.np_desc(a_shape, a_strides, dtype_code, pa)
@@ -298,6 +302,8 @@ def route_pair(a_shape, a_strides, la, b_shape, b_strides, lb, c_shape,
             "launches")
     r = dict(zip(keys, list(out)))
     r["kind"] = ROUTE_KINDS[r["kind"]]
+    if r["kind"] == "stream":
+        r["stream_k"], r["stream_n"] = out[9], out[10]
     return r
 
 

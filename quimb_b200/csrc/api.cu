@@ -111,7 +111,8 @@ static bool want_ozaki(int engine, const PairPlan &plan) {
   if (engine == QB_ENGINE_AUTO) engine = env_engine();
   return engine == QB_ENGINE_OZAKI && ozaki_eligible(plan);
 }
-// streaming engine (contract_stream.cu): small-operator steps, N, K <= 16
+// streaming engine (contract_stream.cu): small-operator steps, N, K <= 32
+// (real) or <= 16 (complex)
 static bool want_stream(int engine, const PairPlan &plan) {
   if (engine == QB_ENGINE_AUTO) engine = env_engine();
   return engine == QB_ENGINE_STREAM && stream_eligible(plan);
@@ -143,7 +144,14 @@ static Route select_route(const PairPlan &plan, int engine) {
     r.launches = 5;  // rowmax + split of each operand, then the int8 GEMM
     return r;
   }
-  if (want_stream(engine, plan)) { r.kind = ROUTE_STREAM; r.launches = 1; return r; }
+  if (want_stream(engine, plan)) {
+    const StreamVariant v = stream_variant(plan.p);
+    r.kind = ROUTE_STREAM;
+    r.launches = 1;
+    r.stream_k = v.kmax;
+    r.stream_n = v.nmax;
+    return r;
+  }
   return dmma_route(plan, true);
 }
 
@@ -180,7 +188,7 @@ int qb_contract_pair_route(const qb_tensor_t *A, const int32_t *la,
   const Route r = select_route(plan, engine & 0xff);
   out[0] = r.kind; out[1] = r.cfg; out[2] = r.splitk; out[3] = r.streamk;
   out[4] = r.sk_head; out[5] = r.bk; out[6] = r.layout; out[7] = sm_count();
-  out[8] = r.launches;
+  out[8] = r.launches; out[9] = r.stream_k; out[10] = r.stream_n;
   return 0;
 }
 
@@ -212,7 +220,9 @@ int qb_debug_contract_stream_host(const qb_tensor_t *A, const int32_t *la,
   }
   plan.p.alpha = alpha; plan.p.beta = beta;
   rc = contract_stream_host(plan);
-  if (rc) set_error("qb_debug_contract_stream_host: needs N, K <= 16 and f64 / c128");
+  if (rc)
+    set_error("qb_debug_contract_stream_host: needs f64 with N, K <= 32 or c128 with "
+              "N, K <= 16");
   return rc;
 }
 

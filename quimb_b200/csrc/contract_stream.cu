@@ -1,7 +1,7 @@
 // Streaming engine for "apply a small operator to a big tensor" contractions:
 //   C[m, n] = alpha * sum_k op(A)[m, k] * op(B)[k, n] + beta * C[m, n]
-// with N <= 16 and K <= 16 (gate application in circuit trees, MPO legs,
-// physical indices: the steps cotengra's pairwise loop issues for
+// with N, K <= 32 (real) or N, K <= 16 (complex) (gate application in
+// circuit trees, MPO legs, physical indices: the steps cotengra's pairwise loop issues for
 // quimb/tensor/circuit/exact.py amplitudes, tensor_core.py:3786-3808).  Such a
 // step moves (M*K + M*N) elements for 2*M*N*K flops -- arithmetic intensity
 // of a few flop/byte, i.e. HBM-bound, and a 128 x 32 DMMA tile would spend
@@ -197,15 +197,24 @@ static int launch_stream_t(const ContractParams &p, cudaStream_t st) {
   return 0;
 }
 
+StreamVariant stream_variant(const ContractParams &p) {
+  if (p.N <= 4 && p.K <= 4) return {4, 4};
+  if (p.N <= 4 && p.K <= 16) return {16, 4};
+  if (p.K <= 4 && p.N <= 16) return {4, 16};
+  if (p.N <= 16 && p.K <= 16) return {16, 16};
+  return {32, 32};
+}
+
 template <bool CPLX>
 static int launch_stream_c(const PairPlan &plan, cudaStream_t st) {
   ContractParams p = plan.p;
   p.splitk = 1;
   p.partial = nullptr;
-  if (p.N <= 4 && p.K <= 4) return launch_stream_t<CPLX, 4, 4>(p, st);
-  if (p.N <= 4 && p.K <= 16) return launch_stream_t<CPLX, 16, 4>(p, st);
-  if (p.K <= 4 && p.N <= 16) return launch_stream_t<CPLX, 4, 16>(p, st);
-  if (p.N <= 16 && p.K <= 16) return launch_stream_t<CPLX, 16, 16>(p, st);
+  const StreamVariant v = stream_variant(p);
+  if (v.kmax == 4 && v.nmax == 4) return launch_stream_t<CPLX, 4, 4>(p, st);
+  if (v.kmax == 16 && v.nmax == 4) return launch_stream_t<CPLX, 16, 4>(p, st);
+  if (v.kmax == 4 && v.nmax == 16) return launch_stream_t<CPLX, 4, 16>(p, st);
+  if (v.kmax == 16 && v.nmax == 16) return launch_stream_t<CPLX, 16, 16>(p, st);
   if constexpr (!CPLX) return launch_stream_t<false, 32, 32>(p, st);
   return -9;
 }
@@ -226,16 +235,17 @@ static void stream_host_t(const ContractParams &p) {
   constexpr int ES = CPLX ? 2 : 1;
   double Bs[32 * 32 * ES];
   int64_t kOffA[32], nOffC[32];
+  const StreamVariant v = stream_variant(p);
   for (int64_t zb = 0; zb < p.nbatch; ++zb) {
     const double *A, *B;
     double *C;
     stream_batch_base<CPLX>(p, zb, A, B, C);
     stream_fill_tables<CPLX>(p, B, 0, 1, Bs, kOffA, nOffC);
     for (int64_t m = 0; m < p.M; ++m) {
-      if (p.N <= 4 && p.K <= 4) stream_row<CPLX, 4, 4>(p, A, C, m, Bs, kOffA, nOffC);
-      else if (p.N <= 4 && p.K <= 16) stream_row<CPLX, 16, 4>(p, A, C, m, Bs, kOffA, nOffC);
-      else if (p.K <= 4 && p.N <= 16) stream_row<CPLX, 4, 16>(p, A, C, m, Bs, kOffA, nOffC);
-      else if (p.N <= 16 && p.K <= 16) stream_row<CPLX, 16, 16>(p, A, C, m, Bs, kOffA, nOffC);
+      if (v.kmax == 4 && v.nmax == 4) stream_row<CPLX, 4, 4>(p, A, C, m, Bs, kOffA, nOffC);
+      else if (v.kmax == 16 && v.nmax == 4) stream_row<CPLX, 16, 4>(p, A, C, m, Bs, kOffA, nOffC);
+      else if (v.kmax == 4 && v.nmax == 16) stream_row<CPLX, 4, 16>(p, A, C, m, Bs, kOffA, nOffC);
+      else if (v.kmax == 16 && v.nmax == 16) stream_row<CPLX, 16, 16>(p, A, C, m, Bs, kOffA, nOffC);
       else stream_row<CPLX, 32, 32>(p, A, C, m, Bs, kOffA, nOffC);
     }
   }

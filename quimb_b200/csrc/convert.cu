@@ -9,23 +9,6 @@ namespace qb {
 
 template <typename S, typename D>
 __global__ void __launch_bounds__(256)
-    convert_strided_kernel(const S *__restrict__ src, D *__restrict__ dst, int64_t n,
-                           int rank, const int64_t *__restrict__ meta) {
-  // meta: shape[rank], src_stride[rank] (elements); dst is contiguous
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    int64_t r = i, off = 0;
-    for (int d = rank - 1; d >= 0; --d) {
-      const int64_t e = meta[d], q = r / e;
-      off += (r - q * e) * meta[rank + d];
-      r = q;
-    }
-    dst[i] = (D)src[off];
-  }
-}
-
-template <typename S, typename D>
-__global__ void __launch_bounds__(256)
     convert_contig_kernel(const S *__restrict__ src, D *__restrict__ dst, int64_t n) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (int64_t)gridDim.x * blockDim.x)

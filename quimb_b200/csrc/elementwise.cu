@@ -28,16 +28,19 @@ struct PermParams {
   int32_t conj;
 };
 
+// Conjugation flips the sign bit of the imaginary part (IEEE negate), so the
+// copy stays bitwise: an arithmetic -x compiles to an add, which replaces a
+// NaN's payload with the canonical NaN.
 template <typename T>
 __device__ __forceinline__ T conj_if(T v, int) { return v; }
 template <>
 __device__ __forceinline__ double2 conj_if(double2 v, int c) {
-  if (c) v.y = -v.y;
+  if (c) v.y = __longlong_as_double(__double_as_longlong(v.y) ^ (long long)(1ULL << 63));
   return v;
 }
 template <>
 __device__ __forceinline__ float2 conj_if(float2 v, int c) {
-  if (c) v.y = -v.y;
+  if (c) v.y = __int_as_float(__float_as_int(v.y) ^ (int)0x80000000u);
   return v;
 }
 

@@ -19,6 +19,12 @@ int launch_contract_ozaki(const PairPlan &plan, void *workspace, cudaStream_t st
 
 // streaming engine for small-operator steps (contract_stream.cu)
 bool stream_eligible(const PairPlan &plan);
+// compiled (KMAX, NMAX) register-array bounds the launch and the host executor
+// pick for an eligible plan; qb_contract_pair_route reports the same pair
+struct StreamVariant {
+  int kmax, nmax;
+};
+StreamVariant stream_variant(const ContractParams &p);
 int launch_contract_stream(const PairPlan &plan, cudaStream_t st);
 int contract_stream_host(const PairPlan &plan);  // TEST: same row code on host pointers
 

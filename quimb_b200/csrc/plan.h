@@ -449,6 +449,8 @@ struct Route {
   int bk;         // DMMA k-block depth
   int layout;     // cfg 0, real: a_kmajor * 2 + b_kmajor; -1: runtime layout
   int launches;   // kernels launched (beta = 0)
+  int stream_k;   // streaming engine: compiled (KMAX, NMAX) variant, 0 otherwise
+  int stream_n;
 };
 
 // DMMA part of a route.  A stream-K grid needs the workspace scratch that the

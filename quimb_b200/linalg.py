@@ -572,7 +572,11 @@ def _svd_complex(x, return_sweeps):
 
 
 def norm(x, ord=None):
-    """Frobenius / 2-norm through the deterministic dot kernel."""
+    """Frobenius / 2-norm through the deterministic dot kernel.
+
+    Known limit: this is sqrt(<x, x>) without scaling, so it overflows to inf
+    for norms above about 2^511 and underflows to 0 below about 2^-537, as
+    numpy's ``norm`` (the reference's) does."""
     x = ops.asarray(x)
     if ord not in (None, "fro", 2):
         raise NotImplementedError("only the Frobenius / vector 2-norm")

@@ -5,9 +5,13 @@ and the reference results the kernels are held to.
 Reference arithmetic is plain numpy in float64.  ``nonfinite_class`` gives the
 IEEE class (NaN / +inf / -inf / finite) of every element of A @ B from the
 positions of the special values alone, so it does not depend on how a BLAS
-treats them."""
+treats them.  ``exact_dot`` is the correctly rounded inner product (products
+split exactly, summed by ``math.fsum``) the vector-kernel tests compare with."""
+
+import math
 
 import numpy as np
+import torch
 
 from quimb_b200 import _lib
 from quimb_b200.contract import route_pair
@@ -31,6 +35,18 @@ FORMS = {
 QB_DTYPE = {"float32": _lib.QB_F32, "float64": _lib.QB_F64,
             "complex64": _lib.QB_C64, "complex128": _lib.QB_C128}
 ENGINE_INT8 = 2
+ENGINE_STREAM = 3
+
+# the streaming engine's compiled (KMAX, NMAX) variants (contract_stream.cu):
+# real operators up to 32 x 32, complex ones up to 16 x 16
+STREAM_VARIANTS = {"float64": ((4, 4), (16, 4), (4, 16), (16, 16), (32, 32)),
+                   "complex128": ((4, 4), (16, 4), (4, 16), (16, 16))}
+# its search grid: every variant at its largest (K, N) and just past the
+# previous variant's limit; M = 3 full 256-row blocks and a ragged one
+STREAM_KN = (1, 4, 5, 16, 17, 32)
+STREAM_M = 3 * 256 + 7
+# zero-fill shapes: contracted extent 0, a 3-element output is the cheapest
+ZERO_FILL_M, ZERO_FILL_N = 3, 5
 
 
 def strides(shape):
@@ -55,9 +71,14 @@ def route_of(form, M, K, N, dtype, engine=0):
 
 def route_key(dtype, r):
     """Identity of a compiled kernel variant: dtype x engine x tile config x
-    {plain, split-K, stream-K} x cfg-0 layout of real operands."""
+    {plain, split-K, stream-K} x cfg-0 layout of real operands; the streaming
+    engine's (KMAX, NMAX) variant; the zero fill and the widening path."""
     if r["kind"] == "int8":
         return (dtype, "int8")
+    if r["kind"] == "stream":
+        return (dtype, "stream", r["stream_k"], r["stream_n"])
+    if r["kind"] in ("zero_fill", "widen"):
+        return (dtype, r["kind"])
     if r["kind"] == "dmma_streamk":
         return (dtype, "streamk", 0, r["layout"])
     if r["kind"] == "dmma":
@@ -69,8 +90,17 @@ def route_key(dtype, r):
 
 def required_keys():
     """Every route qb_contract_pair can dispatch a float64 / complex128
-    contraction to, plus the int8 engine for all four dtypes."""
+    contraction to (DMMA, int8 on request, every streaming variant on
+    request), the int8 engine and the widening path of float32 / complex64,
+    and the zero fill of all four dtypes."""
     keys = set()
+    for dt, variants in STREAM_VARIANTS.items():
+        for k, n in variants:
+            keys.add((dt, "stream", k, n))
+    for dt in QB_DTYPE:
+        keys.add((dt, "zero_fill"))
+    keys.add(("float32", "widen"))
+    keys.add(("complex64", "widen"))
     for dt in ("float64", "complex128"):
         for c in range(1, 5):
             keys.add((dt, "plain", c, -1))
@@ -85,6 +115,15 @@ def required_keys():
     keys.add(("float32", "int8"))
     keys.add(("complex64", "int8"))
     return keys
+
+
+def einsum_spec(la, lb, lc):
+    """numpy einsum subscripts of integer mode labels."""
+    sym = {}
+    for l in list(la) + list(lb) + list(lc):
+        sym.setdefault(l, chr(ord("a") + len(sym)))
+    word = lambda ls: "".join(sym[l] for l in ls)  # noqa: E731
+    return f"{word(la)},{word(lb)}->{word(lc)}"
 
 
 def macs(form, M, K, N, dtype):
@@ -110,7 +149,41 @@ def search_routes():
                     continue
                 if key not in best or cost < best[key][0]:
                     best[key] = (cost, (form, M, K, N, eng, r))
+        for form in FORMS:
+            # contracted extent 0: the cheapest shape has the fewest outputs
+            M, N = ZERO_FILL_M, 1 if form == "ab,b" else ZERO_FILL_N
+            r = route_of(form, M, 0, N, dtype)
+            key = route_key(dtype, r)
+            cost = (GROUPS if form.startswith("g") else 1) * M * N
+            if key is not None and (key not in best or cost < best[key][0]):
+                best[key] = (cost, (form, M, 0, N, 0, r))
+    # streaming variants at their largest operator (then the cheapest form)
+    for key, shapes in stream_shapes().items():
+        best[key] = (None, max(shapes, key=lambda s: (s[2] * s[3], -macs(*s[:4], key[0]))))
     return {k: v[1] for k, v in best.items()}
+
+
+def stream_shapes():
+    """{streaming route key: [(form, M, K, N, engine, route), ...]} over the
+    streaming grid (K, N in STREAM_KN, M = STREAM_M) with the engine
+    requested."""
+    out = {}
+    for dtype in STREAM_VARIANTS:
+        for form in FORMS:
+            for K in STREAM_KN:
+                for N in ((1,) if form == "ab,b" else STREAM_KN):
+                    r = route_of(form, STREAM_M, K, N, dtype, ENGINE_STREAM)
+                    key = route_key(dtype, r)
+                    if key is not None and key[1] == "stream":
+                        out.setdefault(key, []).append((form, STREAM_M, K, N, ENGINE_STREAM, r))
+    return out
+
+
+def stream_lower_edges():
+    """Cheapest shape of every streaming variant: for each variant past the
+    first one, a shape just past the previous variant's limit."""
+    return {key: min(shapes, key=lambda s: macs(*s[:4], key[0]))
+            for key, shapes in stream_shapes().items()}
 
 
 # ---- operand layouts ---------------------------------------------------------
@@ -161,6 +234,64 @@ def pad_spec(shape):
     return [s + p for s, p in zip(shape, pad)], off
 
 
+# ---- device buffers with NaN padding / sentinel bits -----------------------
+TORCH = {"float32": torch.float32, "float64": torch.float64,
+         "complex64": torch.complex64, "complex128": torch.complex128}
+# integer view and sentinel bit pattern (a quiet NaN with a payload) per dtype
+BITS = {"float32": (torch.int32, 0x7FC0BEEF), "complex64": (torch.int32, 0x7FC0BEEF),
+        "float64": (torch.int64, 0x7FF8DEADBEEF0001),
+        "complex128": (torch.int64, 0x7FF8DEADBEEF0001)}
+
+
+def dtype_name(t):
+    return {v: k for k, v in TORCH.items()}[t.dtype]
+
+
+def bits(t):
+    """Integer view of the real parts of `t` (bitwise comparisons)."""
+    r = torch.view_as_real(t) if t.is_complex() else t
+    return r.view(BITS[dtype_name(t)][0])
+
+
+def nan_fill(buf):
+    buf.fill_(float("nan") if not buf.is_complex() else complex(float("nan"), float("nan")))
+    return buf
+
+
+def padded(x, fill_bits=None, transpose=False):
+    """Device view holding numpy `x` inside a larger buffer whose other
+    elements are NaN (inputs) or the sentinel bit pattern (outputs).
+    transpose: the buffer stores the last two axes swapped and the view
+    permutes them back.  Returns (buffer, view, mask of the view's elements)."""
+    dt = str(x.dtype)
+    shape = list(x.shape)
+    if transpose:
+        shape[-2:] = shape[-2:][::-1]
+    bshape, off = pad_spec(shape)
+    buf = torch.empty(bshape, dtype=TORCH[dt], device="cuda")
+    if fill_bits is None:
+        nan_fill(buf)
+    else:
+        bits(buf).fill_(fill_bits)
+    sl = tuple(slice(o, o + s) for o, s in zip(off, shape))
+    view = buf[sl]
+    if transpose:
+        view = view.transpose(-1, -2)
+    view.copy_(torch.from_numpy(np.ascontiguousarray(x)))
+    mask = np.zeros(bshape, dtype=bool)
+    mask[sl] = True
+    return buf, view, mask
+
+
+def assert_sentinel_kept(buf, mask, dtype):
+    """Every element of `buf` outside `mask` still holds the sentinel bits."""
+    b = bits(buf).cpu().numpy()
+    if b.ndim > mask.ndim:
+        mask = np.broadcast_to(mask[..., None], b.shape)
+    outside = b[~mask]
+    assert np.all(outside == BITS[dtype][1]), "a store landed outside the output view"
+
+
 # ---- numbers ---------------------------------------------------------------
 def int_operand(rng, shape, dtype, lim=8):
     """Integer-valued entries in [-lim, lim] (complex: both parts)."""
@@ -183,6 +314,57 @@ def wide(x):
 
 def gamma(n, u=2.0 ** -53):
     return n * u / (1 - n * u)
+
+
+def _veltkamp(x):
+    """x = hi + lo exactly, each part with at most 26 significant bits, so
+    every product of two parts is exact in float64 (x finite, |x| < 2^995)."""
+    c = x * 134217729.0                     # 2^27 + 1
+    hi = c - (c - x)
+    return hi, x - hi
+
+
+def exact_dot(x, y):
+    """sum_i x_i y_i correctly rounded to float64 (real float64 arrays): the
+    products are split into exact sums of two-part products, which
+    ``math.fsum`` adds without intermediate rounding."""
+    x = np.asarray(x, dtype=np.float64).ravel()
+    y = np.asarray(y, dtype=np.float64).ravel()
+    xh, xl = _veltkamp(x)
+    yh, yl = _veltkamp(y)
+    terms = np.concatenate([xh * yh, xh * yl, xl * yh, xl * yl])
+    return math.fsum(terms[terms != 0])
+
+
+def exact_vdot(x, y):
+    """conj(x) . y correctly rounded (per part for complex) and the bound
+    scale sum |terms| of its real products; x, y of any dtype."""
+    x, y = wide(np.asarray(x)).ravel(), wide(np.asarray(y)).ravel()
+    if not np.iscomplexobj(x):
+        return exact_dot(x, y), float(np.sum(np.abs(x * y)))
+    xs, ys = np.concatenate([x.real, x.imag]), np.concatenate([y.real, y.imag])
+    xt, yt = np.concatenate([x.real, -x.imag]), np.concatenate([y.imag, y.real])
+    re, im = exact_dot(xs, ys), exact_dot(xt, yt)
+    return complex(re, im), float(max(np.sum(np.abs(xs * ys)), np.sum(np.abs(xt * yt))))
+
+
+def widen_bound(a, b):
+    """The widening path: the float64 product within ``dmma_bound``, then
+    rounded once to float32 (complex: each part, sqrt(2) u32 |C| in all)."""
+    ref = np.abs(wide(a) @ wide(b))
+    dm = dmma_bound(a, b)
+    u32 = 2.0 ** -24 * (np.sqrt(2) if np.iscomplexobj(a) else 1.0)
+    return dm + u32 * (ref + dm) * 1.001
+
+
+def route_bound(kind, a, b):
+    """Per-element bound of route kind `kind` ("int8", "widen", DMMA and
+    streaming kinds) on C = a @ b against numpy's float64 product."""
+    if kind == "int8":
+        return int8_bound(a, b, a.dtype in (np.float32, np.complex64))
+    if kind == "widen":
+        return widen_bound(a, b)
+    return dmma_bound(a, b)
 
 
 def dmma_bound(a, b):
@@ -274,11 +456,14 @@ def classify(x):
     return cls
 
 
-def check_classes(a, b, got, int8):
+def check_classes(a, b, got, int8=False, kind=None):
     """got (float64 / complex128, [G, M, N]) against a @ b with special values
     in a, b ([G, M, K], [G, K, N]): the IEEE class of every element, and the
     finite elements -- outputs of rows and columns without special values --
-    within the bound of the engine."""
+    within the bound of route kind `kind` (see ``route_bound``; without it,
+    the int8 engine's bound when `int8`, else the DMMA bound)."""
+    if kind is None:
+        kind = "int8" if int8 else "dmma"
     for g in range(a.shape[0]):
         want = nonfinite_class(wide(a[g]), wide(b[g]))
         if np.iscomplexobj(got):
@@ -290,8 +475,7 @@ def check_classes(a, b, got, int8):
     b0 = np.where(np.isfinite(b), b, 0)
     fin = np.isfinite(got)
     ref = wide(a0) @ wide(b0)
-    single = a.dtype in (np.float32, np.complex64)
-    bound = int8_bound(a0, b0, single) if int8 else dmma_bound(a0, b0)
+    bound = route_bound(kind, a0, b0)
     assert np.all(np.abs(got[fin] - ref[fin]) <= bound[fin])
 
 

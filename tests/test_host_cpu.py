@@ -476,3 +476,79 @@ def test_decomposition_oracle_is_exact():
     np.testing.assert_allclose(do.mp_svd(B), np.linalg.svd(B, compute_uv=False), rtol=1e-13)
     r = np.linalg.qr(B)[1]
     np.testing.assert_allclose(do.mp_qr_r(B), r * np.sign(np.diag(r))[:, None], atol=1e-13)
+
+
+def test_route_pins_every_stream_variant():
+    """The streaming engine's compiled (KMAX, NMAX) variant in the route
+    report: one shape per variant, each at a limit, and the DMMA fallback of
+    shapes past a variant's reach (complex operators past 16, real past 32)."""
+    from tests import route_oracle as ro
+    S = ro.ENGINE_STREAM
+
+    def rk(K, N, dt="float64"):
+        r = ro.route_of("ab,bc", ro.STREAM_M, K, N, dt, S)
+        return r["kind"], r.get("stream_k", 0), r.get("stream_n", 0)
+
+    for dt in ("float64", "complex128"):
+        assert rk(4, 4, dt) == ("stream", 4, 4)
+        assert rk(5, 4, dt) == ("stream", 16, 4)
+        assert rk(16, 1, dt) == ("stream", 16, 4)
+        assert rk(4, 5, dt) == ("stream", 4, 16)
+        assert rk(1, 16, dt) == ("stream", 4, 16)
+        assert rk(5, 5, dt) == ("stream", 16, 16)
+        assert rk(16, 16, dt) == ("stream", 16, 16)
+    assert rk(17, 1) == ("stream", 32, 32)
+    assert rk(32, 32) == ("stream", 32, 32)
+    for K, N in ((17, 4), (4, 17), (17, 17), (32, 32)):
+        assert rk(K, N, "complex128") == ("dmma", 0, 0)
+    assert rk(33, 4) == ("dmma", 0, 0)
+    # without the request the same shape takes DMMA and reports no variant,
+    # neither in the C report's slots nor as keys of the Python dict
+    r = ro.route_of("ab,bc", ro.STREAM_M, 16, 16, "float64")
+    assert r["kind"] == "dmma" and "stream_k" not in r and "stream_n" not in r
+    sa, sb, sc = [ro.STREAM_M, 16], [16, 16], [ro.STREAM_M, 16]
+    out = (ctypes.c_int64 * 16)(*([-7] * 16))
+    for eng, want in ((0, (0, 0)), (S, (16, 16))):
+        rc = _lib.load().qb_contract_pair_route(
+            _lib.np_desc(sa, _strides(sa), _lib.QB_F64), _lib.labels([0, 1]),
+            _lib.np_desc(sb, _strides(sb), _lib.QB_F64), _lib.labels([1, 2]),
+            _lib.np_desc(sc, _strides(sc), _lib.QB_F64), _lib.labels([0, 2]), eng, out)
+        assert rc == 0 and (out[9], out[10]) == want
+
+
+def test_stream_route_search_reaches_every_variant():
+    """The streaming grid reaches all 9 variants, each at its largest
+    operator, with a lower-edge shape just past the previous variant."""
+    from tests import route_oracle as ro
+    want = {(dt, "stream", k, n) for dt, vs in ro.STREAM_VARIANTS.items() for k, n in vs}
+    assert len(want) == 9
+    found = ro.stream_shapes()
+    assert set(found) == want
+    top = ro.search_routes()
+    low = ro.stream_lower_edges()
+    for key in want:
+        _, _, K, N, _, _ = top[key]
+        assert (K, N) == key[2:], (key, K, N)
+        _, _, K, N, _, _ = low[key]
+        assert max(K, N) in (1, 5, 17), (key, K, N)
+
+
+def test_exact_dot_reference_is_correctly_rounded():
+    """route_oracle.exact_dot against rational arithmetic: the correctly
+    rounded value of sum x_i y_i for random pairs of wide dynamic range."""
+    from fractions import Fraction
+    from tests import route_oracle as ro
+    rng = np.random.default_rng(7)
+    for trial in range(300):
+        n = int(rng.integers(1, 40))
+        x = np.ldexp(rng.standard_normal(n), rng.integers(-60, 60, size=n))
+        y = np.ldexp(rng.standard_normal(n), rng.integers(-60, 60, size=n))
+        if trial % 3 == 0:                 # heavy cancellation
+            y[-1] = -float(np.dot(x[:-1], y[:-1])) / x[-1]
+        exact = sum(Fraction(a) * Fraction(b) for a, b in zip(x.tolist(), y.tolist()))
+        got = ro.exact_dot(x, y)
+        assert Fraction(got) == Fraction(float(exact)), (trial, got, float(exact))
+    z = rng.standard_normal(8) + 1j * rng.standard_normal(8)
+    w = rng.standard_normal(8) + 1j * rng.standard_normal(8)
+    got, scale = ro.exact_vdot(z, w)
+    assert abs(got - np.vdot(z, w)) <= 1e-14 * scale
