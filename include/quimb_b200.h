@@ -346,9 +346,17 @@ int qb_svals_to_keep(const double *s, int64_t n, double cutoff,
  * qb_p2p_free), exports it (64-byte CUDA IPC handle) and imports the blocks
  * of its peers; `peer_bufs[world]` lists the block bases in rank order, the
  * caller's own block at index `rank`.  `epoch` counts the calls of each kind
- * (1, 2, ...; the same sequence on every rank); `scratch` is 8 bytes of
- * zeroed device memory (CTA counter, error word: non-zero after a kernel gave
- * up waiting ~4 s for a peer).
+ * (1, 2, ...; the same sequence on every rank; epoch 0 is rejected because
+ * the flags start at 0); `scratch` is 8 bytes of zeroed device memory (CTA
+ * counter, error word: non-zero after a kernel gave up waiting ~4 s for a
+ * peer).  Every accepted call launches exactly one kernel.
+ *
+ * Error codes of the two exchange calls (nothing is launched): -1 world or
+ * rank out of range (at most 16 ranks), -2 null peer block, -3 null scratch,
+ * -4 epoch 0, -5 bad slab / vector (negative, not 16-byte granular or
+ * aligned, null; for the all-reduce m outside [0, 64] or x not 8-byte
+ * aligned), -6 slab past the gather buffer (dst_off + bytes above
+ * gather_bytes rounded up to 256).
  */
 int64_t qb_p2p_block_bytes(int64_t gather_bytes);
 int64_t qb_p2p_data_offset(int64_t gather_bytes, int parity);
@@ -359,11 +367,15 @@ int qb_p2p_import(const unsigned char *handle64, void **peer_ptr);
 int qb_p2p_unimport(void *peer_ptr);
 /* all ranks: slab `x` (bytes, 16-byte granular) -> byte offset dst_off of the
  * gather buffer of parity (epoch & 1) on EVERY rank; when the kernel has
- * completed the whole vector is resident in the local block. */
+ * completed the whole vector is resident in the local block.  An empty slab
+ * (bytes == 0, x may be null) is legal and still raises this rank's flags. */
 int qb_p2p_allgather(void *const *peer_bufs, int world, int rank, const void *x,
                      int64_t bytes, int64_t dst_off, int64_t gather_bytes,
                      uint64_t epoch, void *scratch, void *stream);
-/* in-place sum over the ranks of m <= 64 doubles, bit-identical everywhere */
+/* in-place sum over the ranks of m <= 64 doubles, bit-identical everywhere:
+ * x[t] = ((p_0 + p_1) + p_2) + ... in rank order from rank 0's partial, so one
+ * rank is the identity and -0.0 partials sum to -0.0.  Every rank passes the
+ * same m; m == 0 still launches and raises the epoch's flags. */
 int qb_p2p_allreduce_small(void *const *peer_bufs, int world, int rank, void *x,
                            int m, uint64_t epoch, void *scratch, void *stream);
 

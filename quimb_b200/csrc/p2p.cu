@@ -137,9 +137,11 @@ __global__ void __launch_bounds__(64)
   __syncthreads();
   if (t < m) {
     const double *s = reinterpret_cast<const double *>(
-        static_cast<const char *>(P.buf[P.rank]) + slot);
-    double acc = 0.0;
-    for (int r = 0; r < P.world; ++r) acc += __ldcg(s + r * P2P_RMAX + t);  // L2, fixed order
+        static_cast<const char *>(P.buf[P.rank]) + slot) + t;
+    // start from rank 0's value, not from +0.0: one rank is the identity and
+    // a sum of -0.0 partials stays -0.0 (IEEE addition of the partials)
+    double acc = __ldcg(s);
+    for (int r = 1; r < P.world; ++r) acc += __ldcg(s + r * P2P_RMAX);  // L2, fixed order
     x[t] = acc;
   }
 }
@@ -210,30 +212,55 @@ int qb_p2p_unimport(void *peer_ptr) {
   return 0;
 }
 
+// Checks shared by both entry points: -3 null scratch, -4 epoch 0 (the flags
+// start at 0, so a wait for epoch 0 would pass before any peer has stored).
+static int check_epoch_scratch(const char *fn, uint64_t epoch, const void *scratch) {
+  if (!scratch) {
+    set_error("%s: scratch is null (8 bytes of zeroed device memory)", fn);
+    return -3;
+  }
+  if (epoch == 0) {
+    set_error("%s: epoch must be >= 1 (flags start at 0)", fn);
+    return -4;
+  }
+  return 0;
+}
+
 // Push `bytes` (multiple of 16, 16-byte aligned source) from x into every
 // rank's gather buffer at byte offset dst_off; returns when the kernel is
 // enqueued.  After the kernel the full gathered vector of this epoch sits at
 // qb_p2p_data_offset(gather_bytes, epoch & 1) of the LOCAL block.
 // `scratch` = 8 bytes of zero-initialised device memory (CTA counter + error
-// word) owned by the caller.
+// word) owned by the caller.  An empty slab (bytes == 0) still launches one
+// CTA: it raises this rank's flags and waits for the peers' like any other.
 int qb_p2p_allgather(void *const *peer_bufs, int world, int rank, const void *x,
                      int64_t bytes, int64_t dst_off, int64_t gather_bytes,
                      uint64_t epoch, void *scratch, void *stream) {
   P2PPeers P;
   int rc = fill_peers(P, peer_bufs, world, rank);
   if (rc) return rc;
+  rc = check_epoch_scratch("qb_p2p_allgather", epoch, scratch);
+  if (rc) return rc;
+  if (bytes < 0 || dst_off < 0) {
+    set_error("qb_p2p_allgather: negative slab size %lld or offset %lld", (long long)bytes,
+              (long long)dst_off);
+    return -5;
+  }
   if (bytes % 16 || dst_off % 16 || (reinterpret_cast<uintptr_t>(x) & 15)) {
     set_error("qb_p2p_allgather: slab must be 16-byte aligned and a multiple of 16 bytes");
     return -5;
   }
-  const int64_t g = (gather_bytes + 255) / 256 * 256;
-  if (dst_off + bytes > g || !scratch) {
+  if (bytes > 0 && !x) {
+    set_error("qb_p2p_allgather: slab of %lld bytes at a null pointer", (long long)bytes);
+    return -5;
+  }
+  const int64_t g = gather_bytes < 0 ? -1 : (gather_bytes + 255) / 256 * 256;
+  if (g < 0 || bytes > g || dst_off > g - bytes) {
     set_error("qb_p2p_allgather: slab exceeds the gather buffer");
     return -6;
   }
-  if (bytes == 0) return 0;
   const int64_t n16 = bytes / 16;
-  int blocks = (int)std::min<int64_t>((n16 + 511) / 512, sm_count());
+  int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((n16 + 511) / 512, sm_count()));
   unsigned int *counter = static_cast<unsigned int *>(scratch);
   int *err = reinterpret_cast<int *>(counter + 1);
   allgather_push_kernel<<<blocks, 512, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -248,11 +275,18 @@ int qb_p2p_allreduce_small(void *const *peer_bufs, int world, int rank, void *x,
   P2PPeers P;
   int rc = fill_peers(P, peer_bufs, world, rank);
   if (rc) return rc;
-  if (m < 0 || m > P2P_RMAX || !scratch) {
-    set_error("qb_p2p_allreduce_small: m = %d exceeds %d", m, P2P_RMAX);
+  rc = check_epoch_scratch("qb_p2p_allreduce_small", epoch, scratch);
+  if (rc) return rc;
+  if (m < 0 || m > P2P_RMAX) {
+    set_error("qb_p2p_allreduce_small: m = %d outside [0, %d]", m, P2P_RMAX);
     return -5;
   }
-  if (m == 0) return 0;
+  if (m > 0 && (!x || (reinterpret_cast<uintptr_t>(x) & 7))) {
+    set_error("qb_p2p_allreduce_small: x must be a non-null, 8-byte aligned double array");
+    return -5;
+  }
+  // m == 0 still launches and raises the epoch's flags: a skipped epoch would
+  // let the next one reuse the slot parity a slow peer may still be reading
   int *err = reinterpret_cast<int *>(static_cast<unsigned int *>(scratch) + 1);
   allreduce_small_kernel<<<1, 64, 0, static_cast<cudaStream_t>(stream)>>>(
       P, static_cast<double *>(x), m, (unsigned long long)epoch, err);

@@ -336,8 +336,10 @@ class BondShard:
     def all_gather_rows(self, local, n, transient=False):
         """Concatenate the row slabs ``local`` (rows_r, cols) of all ranks into
         the full (n, cols) matrix, identical on every rank.  ``transient``: the
-        caller consumes the result before the next-but-one gather, so the p2p
-        path may return a view of its gather buffer instead of a copy."""
+        caller consumes the result before the next gather is enqueued on this
+        stream, so the p2p path may return a view of its gather buffer instead
+        of a copy.  (Once this rank's next gather has run, a peer may start the
+        one after it, whose push overwrites the buffer of the view.)"""
         cols = local.shape[1]
         if not self.active:
             return local

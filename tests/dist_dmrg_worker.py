@@ -28,6 +28,8 @@ def main():
     ap.add_argument("--L", type=int, default=10)
     ap.add_argument("--chi", type=int, default=24)
     ap.add_argument("--dtype", default="float64")
+    ap.add_argument("--exchange", default="auto",
+                    help="BondShard exchange; 'p2p' runs the peer-memory kernels over CUDA IPC")
     ap.add_argument("--emulate", action="store_true",
                     help="CPU tier: host layer on tests/abi_emulator.py (no device)")
     args = ap.parse_args()
@@ -51,11 +53,20 @@ def run(args, rank, world):
     from oracle import dmrg_np as dm
 
     mpo = dm.mpo_heis(args.L)
-    sh = BondShard()
+    sh = BondShard(exchange=args.exchange)
     ds = qb.DMRG2(mpo, [8, args.chi], cutoffs=1e-12, mpo_shape="lrdu", seed=5,
                   dtype=args.dtype, shard=sh)
     ds.shard_min_bond = 2            # shard every bond >= 2 * world rows
     ds.solve(tol=1e-9, max_sweeps=6)
+    p2p_ok = True
+    if args.exchange == "p2p":
+        # the kernels carried (some of) the exchange and never timed out
+        p2p_ok = sh.exchange_name.startswith("p2p") and sh._px is not None
+        sh.check()
+        if rank == 0:
+            print(f"exchange={sh.exchange_name} p2p gathers={sh._px.g_epoch if sh._px else 0} "
+                  f"reductions={sh._px.r_epoch if sh._px else 0}")
+        sh.close()
     d1 = qb.DMRG2(mpo, [8, args.chi], cutoffs=1e-12, mpo_shape="lrdu", seed=5,
                   dtype=args.dtype)
     d1.solve(tol=1e-9, max_sweeps=6)
@@ -63,7 +74,7 @@ def run(args, rank, world):
     ok = abs(ds.energy - d1.energy) < 1e-8
     if e0 is not None:
         ok = ok and abs(ds.energy - e0) < 1e-6
-    ok = ok and sh.bytes_gathered > 0
+    ok = ok and sh.bytes_gathered > 0 and p2p_ok
     # the replicated part of the sweep stays bit-identical on all ranks
     cdev = "cuda" if args.backend == "nccl" else "cpu"   # NCCL reduces device tensors only
     chk = torch.stack([a.t.abs().sum().double() for a in ds.state]).to(cdev)

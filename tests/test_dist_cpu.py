@@ -4,6 +4,7 @@ stand-in for the device contraction (the product has no CPU arithmetic)."""
 
 import os
 import sys
+import time
 
 import numpy as np
 import pytest
@@ -12,6 +13,31 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def _run_ranks(target, port, timeout, world=2):
+    """Run ``target(rank, world, port, ret)`` in ``world`` spawned processes
+    and return ``ret`` (rank -> result).  Asserts that every rank exited 0 within
+    ``timeout`` seconds; a rank still running then is killed and reaped."""
+    mp.set_start_method("spawn", force=True)
+    mgr = mp.Manager()
+    ret = mgr.dict()
+    procs = [mp.Process(target=target, args=(r, world, port, ret)) for r in range(world)]
+    for p in procs:
+        p.start()
+    deadline = time.monotonic() + timeout
+    try:
+        for p in procs:
+            p.join(timeout=max(0.0, deadline - time.monotonic()))
+    finally:
+        for p in procs:
+            if p.is_alive():
+                p.kill()
+            p.join()
+    assert [p.exitcode for p in procs] == [0] * world
+    out = dict(ret)
+    mgr.shutdown()
+    return out
 
 
 def _np_contract(arrays, inputs, output, optimize):
@@ -64,16 +90,7 @@ def _worker(rank, world, port, ret):
 
 
 def test_slice_parallel_contraction_gloo_world2():
-    mp.set_start_method("spawn", force=True)
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    port = 29500 + (os.getpid() % 2000)
-    procs = [mp.Process(target=_worker, args=(r, 2, port, ret)) for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    ret = _run_ranks(_worker, 29500 + (os.getpid() % 2000), timeout=120)
     assert ret[0][0] and ret[1][0]
     assert ret[0][1] and ret[1][1]
     assert ret[0][2] + ret[1][2] == 15 and abs(ret[0][2] - ret[1][2]) <= 1
@@ -119,16 +136,7 @@ def _shard_worker(rank, world, port, ret):
 
 
 def test_bond_shard_gloo_world2():
-    mp.set_start_method("spawn", force=True)
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    port = 31500 + (os.getpid() % 2000)
-    procs = [mp.Process(target=_shard_worker, args=(r, 2, port, ret)) for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    ret = _run_ranks(_shard_worker, 31500 + (os.getpid() % 2000), timeout=120)
     assert ret[0] and ret[1]
 
 
@@ -162,16 +170,7 @@ def _boundary_worker(rank, world, port, ret):
 
 
 def test_two_sided_boundary_contraction_gloo_world2():
-    mp.set_start_method("spawn", force=True)
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    port = 33500 + (os.getpid() % 2000)
-    procs = [mp.Process(target=_boundary_worker, args=(r, 2, port, ret)) for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(timeout=240)
-        assert p.exitcode == 0
+    ret = _run_ranks(_boundary_worker, 33500 + (os.getpid() % 2000), timeout=240)
     assert ret[0] and ret[1]
 
 
@@ -197,16 +196,7 @@ def _two_ended_worker(rank, world, port, ret):
 
 
 def test_two_ended_mps_norm_gloo_world2():
-    mp.set_start_method("spawn", force=True)
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    port = 35500 + (os.getpid() % 2000)
-    procs = [mp.Process(target=_two_ended_worker, args=(r, 2, port, ret)) for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(timeout=240)
-        assert p.exitcode == 0
+    ret = _run_ranks(_two_ended_worker, 35500 + (os.getpid() % 2000), timeout=240)
     assert ret[0] and ret[1]
 
 
@@ -254,17 +244,7 @@ def _sharded_lanczos_worker(rank, world, port, ret):
 
 
 def test_sharded_lanczos_gloo_world2():
-    mp.set_start_method("spawn", force=True)
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    port = 37500 + (os.getpid() % 2000)
-    procs = [mp.Process(target=_sharded_lanczos_worker, args=(r, 2, port, ret))
-             for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(timeout=240)
-        assert p.exitcode == 0
+    ret = _run_ranks(_sharded_lanczos_worker, 37500 + (os.getpid() % 2000), timeout=240)
     assert ret[0] and ret[1]
 
 
@@ -273,11 +253,8 @@ def test_bond_sharded_dmrg2_gloo_world2_emulated():
     Lanczos + replicated SVD / environments) on gloo with two ranks: energies
     equal the unsharded run and exact diagonalisation, states bit-identical on
     both ranks.  Host layer on the ABI emulator, exchange layer real."""
-    import subprocess
-    port = 39500 + (os.getpid() % 2000)
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2",
-           "--master-addr", "127.0.0.1", "--master-port", str(port),
-           os.path.join(ROOT, "tests", "dist_dmrg_worker.py"), "--backend", "gloo",
-           "--emulate", "--L", "10", "--chi", "20"]
-    pr = subprocess.run(cmd, capture_output=True, text=True, timeout=600, cwd=ROOT)
-    assert "DIST_DMRG_OK" in pr.stdout, pr.stdout[-2000:] + pr.stderr[-2000:]
+    from tests.test_gpu_p2p import run_process_group, torchrun_cmd
+    rc, out, err = run_process_group(
+        torchrun_cmd("dist_dmrg_worker.py", 2, "--backend", "gloo", "--emulate",
+                     "--L", "10", "--chi", "20"), timeout=600)
+    assert rc == 0 and "DIST_DMRG_OK" in out, out[-2000:] + err[-2000:]

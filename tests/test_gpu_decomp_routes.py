@@ -20,7 +20,6 @@ subprocess runs with the Jacobi switches that are read once per process.
 
 import ctypes
 import os
-import subprocess
 import sys
 import textwrap
 import zlib
@@ -32,6 +31,7 @@ import torch
 import quimb_b200 as qb
 from quimb_b200 import _lib, linalg
 from tests import decomp_oracle as do
+from tests.test_gpu_p2p import run_process_group
 
 pytestmark = pytest.mark.gpu
 
@@ -490,8 +490,9 @@ def _run_switched(tmp_path, env_extra):
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     path = str(tmp_path / f"out_{len(env_extra)}_{'_'.join(env_extra)}.npz")
     env = dict(os.environ, **env_extra)
-    subprocess.run([sys.executable, "-c", _SCRIPT.format(root=root, path=path)], env=env,
-                   check=True, timeout=600)
+    rc, _, err = run_process_group([sys.executable, "-c", _SCRIPT.format(root=root, path=path)],
+                                   timeout=600, env=env)
+    assert rc == 0, err[-3000:]
     return dict(np.load(path))
 
 

@@ -154,22 +154,24 @@ def test_lanczos_complex_hermitian():
     assert np.linalg.norm(M @ xv - theta * xv) < 1e-6
 
 
-@pytest.mark.parametrize("dtype", ["float64", "complex128"])
-def test_bond_sharded_eigensolve_two_ranks_one_gpu(dtype):
+@pytest.mark.parametrize("dtype,exchange", [("float64", "auto"), ("complex128", "auto"),
+                                            ("float64", "p2p")],
+                         ids=["float64", "complex128", "float64-p2p"])
+def test_bond_sharded_eigensolve_two_ranks_one_gpu(dtype, exchange):
     """SURVEY 8e: the local eigensolve row-sharded over 2 ranks (both on this
-    GPU, gloo collectives staged through the host) reproduces the unsharded
-    DMRG2 and exact diagonalisation; replicated parts stay bit-identical."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    port = 23000 + (os.getpid() % 4000) + (7 if dtype == "complex128" else 0)
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2",
-           "--master-addr", "127.0.0.1", "--master-port", str(port),
-           os.path.join(root, "tests", "dist_dmrg_worker.py"), "--backend", "gloo",
-           "--same-gpu", "--dtype", dtype]
-    pr = subprocess.run(cmd, capture_output=True, text=True, timeout=300, cwd=root)
-    assert "DIST_DMRG_OK" in pr.stdout, pr.stdout[-2000:] + pr.stderr[-2000:]
+    GPU) reproduces the unsharded DMRG2 and exact diagonalisation; replicated
+    parts stay bit-identical.  'auto' stages the gloo collectives through the
+    host; 'p2p' runs the float64 gathers and reductions in the peer-memory
+    kernels over CUDA IPC (other dtypes never take them)."""
+    import time
+
+    from tests.test_gpu_p2p import run_process_group, torchrun_cmd
+    t0 = time.time()
+    rc, out, err = run_process_group(
+        torchrun_cmd("dist_dmrg_worker.py", 2, "--backend", "gloo", "--same-gpu",
+                     "--dtype", dtype, "--exchange", exchange), timeout=300)
+    print(f"sharded DMRG2 ({dtype}, {exchange}): {time.time() - t0:.1f} s wall")
+    assert rc == 0 and "DIST_DMRG_OK" in out, out[-2000:] + err[-2000:]
 
 
 def test_environments_and_moving_environment_vs_oracle():

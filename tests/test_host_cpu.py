@@ -408,6 +408,56 @@ def test_svd_trunc_and_p2p_argument_errors_without_a_device():
     assert lib.qb_p2p_allgather(bufs, 40, 0, None, 16, 0, 1024, 1, None, None) == -1  # world > 16
 
 
+def test_p2p_exchange_argument_errors_without_a_device():
+    """Every malformed exchange call is refused with its own negative code
+    before any CUDA call.  The pointers are dummies that are never touched, and
+    nothing is launched."""
+    lib = _lib.load()
+    vp = ctypes.c_void_p
+    peers = (vp * 17)(*([0x7f0000000000] * 17))
+    x, scratch = 0x7f1000000000, 0x7f2000000000
+    n0 = _lib.launch_count()
+
+    def ag(world=2, rank=0, x=x, nbytes=256, dst_off=0, gather=1000, epoch=1, scratch=scratch,
+           bufs=peers):
+        return lib.qb_p2p_allgather(bufs, world, rank, vp(x), nbytes, dst_off, gather, epoch,
+                                    vp(scratch), None)
+
+    def ar(world=2, rank=0, x=x, m=24, epoch=1, scratch=scratch, bufs=peers):
+        return lib.qb_p2p_allreduce_small(bufs, world, rank, vp(x), m, epoch, vp(scratch), None)
+
+    def refused(rc, code, fragment):
+        assert rc == code, (rc, code, _lib.last_error())
+        assert fragment in _lib.last_error(), _lib.last_error()
+
+    for call in (ag, ar):
+        for world in (0, 17):
+            refused(call(world=world), -1, "out of range")
+        for rank in (-1, 2):
+            refused(call(rank=rank), -1, "out of range")
+        holes = (vp * 2)(0x7f0000000000, None)
+        refused(call(bufs=holes), -2, "null peer buffer 1")
+        refused(call(scratch=0), -3, "scratch is null")
+        refused(call(epoch=0), -4, "epoch must be >= 1")
+    refused(ag(x=x + 8), -5, "16-byte aligned")
+    refused(ag(nbytes=264), -5, "multiple of 16")
+    refused(ag(dst_off=8), -5, "16-byte aligned")
+    for nbytes, dst_off in ((-16, 0), (-256, 512), (16, -16), (256, -65536)):
+        refused(ag(nbytes=nbytes, dst_off=dst_off), -5, "negative")
+    refused(ag(x=0, nbytes=16), -5, "null pointer")
+    # the gather buffer is gather_bytes rounded up to 256: 1000 -> 1024
+    refused(ag(nbytes=1040), -6, "exceeds the gather buffer")
+    refused(ag(nbytes=16, dst_off=1024), -6, "exceeds the gather buffer")
+    refused(ag(nbytes=512, dst_off=528), -6, "exceeds the gather buffer")
+    refused(ag(nbytes=16, dst_off=(1 << 62)), -6, "exceeds the gather buffer")
+    refused(ag(gather=-256, nbytes=0), -6, "exceeds the gather buffer")
+    for m in (-1, 65):
+        refused(ar(m=m), -5, "outside [0, 64]")
+    refused(ar(x=x + 4), -5, "8-byte aligned")
+    refused(ar(x=0), -5, "non-null")
+    assert _lib.launch_count() == n0
+
+
 def test_path_to_sequence_linear_and_ssa():
     from quimb_b200.compressed import path_to_sequence
     # linear (opt_einsum) path over 4 tensors: contract (0,1) -> appended; then (0,1) again ...
