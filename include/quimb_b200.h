@@ -22,6 +22,10 @@
  *                            (quimb_b200/lanczos.py) -- there is no qb_lanczos_*
  *                            and no plan_create/execute/destroy entry: cached
  *                            chains are CUDA graphs captured by the host layer
+ *   qb_sample_select      <- the per-site probability / choice / projection of
+ *                            MatrixProductState.sample_configuration,
+ *                            quimb/tensor/tn1d/core.py:3871-3990, for a whole
+ *                            batch of samples at once
  *
  * Conventions
  *   - plain C, no C++/torch types; device pointers are borrowed, never freed
@@ -331,6 +335,27 @@ int qb_svals_to_keep(const double *s, int64_t n, double cutoff,
                      int cutoff_mode, int64_t max_bond, int renorm,
                      int64_t *n_keep, double *renorm_factor,
                      double *trunc_error);
+
+/* ---- MPS sampling ------------------------------------------------------- */
+/*
+ * One site of batched MPS sampling, the selection after the contraction
+ * W = V . A_i (MatrixProductState.sample / sample_configuration,
+ * quimb/tensor/tn1d/core.py:3871-3990).  W is C x d x r, contiguous, of
+ * dtype QB_F64 or QB_C128 (16-byte aligned for complex).  For every sample c:
+ *   pi[s] = sum_j |W[c, s, j]|^2 (fp64), p = pi / sum(pi) with numpy's
+ *   pairwise sum, cdf = cumsum(p) / cdf[d-1], x = #{s : cdf[s] <= u[c*ldu]}
+ *   (numpy's Generator.choice(d, p=p) for the uniform u: searchsorted
+ *   side='right'; a zero-probability outcome is never chosen),
+ *   config[c*ldc] = x, omega[c] *= p[x], V[c, :] = W[c, x, :] / sqrt(pi[x])
+ *   (C x r, contiguous: the selected row at unit norm).
+ * A row whose sum(pi) is zero or not finite, or whose u lies outside [0, 1),
+ * gets config = -1, omega = NaN and a zero V row.  The arithmetic of a row
+ * depends on d and r only (never on C or the launch shape).  1 <= d <= 256
+ * (-3 otherwise), r >= 1; C == 0 launches nothing.  One launch.
+ */
+int qb_sample_select(int dtype, int64_t C, int64_t d, int64_t r, const void *W,
+                     const double *u, int64_t ldu, int64_t *config, int64_t ldc,
+                     double *omega, void *V, void *stream);
 
 /* ---- device queries / microbenchmarks ---------------------------------- */
 /* ------------------------------------------------------------------------

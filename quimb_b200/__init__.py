@@ -35,7 +35,8 @@ from .split import (array_split, array_svals, cholesky_regularized,  # noqa: F40
 from .lanczos import eigh_lanczos  # noqa: F401
 from . import boundary, linop, tebd, treeopt  # noqa: F401
 from .linop import TNLinearOperator  # noqa: F401
-from .tebd import TEBD, LocalHam1D, gate_split, gate_with_auto_swap  # noqa: F401
+from .tebd import (TEBD, LocalHam1D, gate_split, gate_with_auto_swap,  # noqa: F401
+                   mps_sample, mps_sample_configuration)
 from .boundary import (BoundaryContractor2D, contract_boundary,  # noqa: F401
                        contract_boundary_two_sided, peps_norm_tensors)
 from .dmrg import DMRG1, DMRG2  # noqa: F401

@@ -9,6 +9,7 @@ Mirrors, at array level and for open boundaries,
   LocalHam1D (nearest neighbour) tn1d/tebd.py:12-96, tnag/tebd.py:180-392
   trotter_schedule               tnag/tebd.py:78-126
   TEBD.sweep / step / update_to  tn1d/tebd.py:221-553
+  MatrixProductState.sample      tn1d/core.py:3871-3990 (all samples at once)
 
 MPS sites are (l, p, r) device arrays.  One gate application is a 3-tensor
 contraction (two launches of the pairwise kernel, gate indices folded into
@@ -403,6 +404,144 @@ def mps_amplitude(sites, bits):
         M = Array(A.t[:, int(b), :], A.cj)
         v = M if v is None else ops.tensordot(v, M, axes=((v.ndim - 1,), (0,)))
     return v.reshape(()).item()
+
+
+# ---------------------------------------------------------------- sampling ---
+# Byte budget of one chunk's W = V . A_i (C_chunk x d x r): samples are drawn
+# in chunks small enough for W to stay below it.
+SAMPLE_CHUNK_BYTES = 1 << 30
+
+
+def _sample_rng(seed):
+    """numpy Generator of ``seed``: an int / None seeds a new one, a Generator
+    (or a ``quimb_b200.random.default_rng`` wrapper of one) is used as is."""
+    if hasattr(seed, "_rng"):
+        seed = seed._rng
+    return np.random.default_rng(seed)
+
+
+def _sample_prepare(sites):
+    """Right-canonical, unit-norm fp64 / c128 copy of an open-boundary MPS
+    (the caller's list and arrays are not touched) and the norm factor taken
+    off its first site, a 0-d device array."""
+    sites = [ops.asarray(a) for a in sites]
+    if not sites:
+        raise ValueError("mps_sample: empty MPS")
+    for a in sites:
+        if a.ndim != 3:
+            raise ValueError("mps_sample: sites must be (l, p, r) arrays")
+        if np.dtype(a.dtype).kind not in "fc":
+            raise TypeError(f"mps_sample: unsupported dtype {a.dtype}")
+    if sites[0].shape[0] != 1 or sites[-1].shape[2] != 1:
+        raise ValueError("mps_sample: open boundaries only (first left and last "
+                         "right bond of dimension 1)")
+    from .contract import _WIDE, convert
+    cplx = any(np.dtype(a.dtype).kind == "c" for a in sites)
+    psi = []
+    for a in sites:
+        if cplx and np.dtype(a.dtype).kind == "f":
+            a = a.astype(np.complex128 if a.dtype == np.float64 else np.complex64)
+        if a.t.dtype in _WIDE:
+            # single precision: widen once, sample in double precision
+            a = Array(convert(ops.materialize(a).t, _WIDE[a.t.dtype]))
+        psi.append(a)
+    canonicalize(psi, 0)
+    # the centre to unit norm through an LQ of the 1 x (d r) site: the QR
+    # kernel rescales by a power of two, so norms of 1e+-200 neither overflow
+    # nor underflow; L (1 x 1) is the norm
+    A = psi[0]
+    _, d, r = A.shape
+    Lf, _, Q = qr_stabilized(A.reshape(1, d * r), absorb=get_Us_VH)
+    psi[0] = ops.materialize(Q).reshape(1, d, r)
+    return psi, Lf.reshape(())
+
+
+def _sample_chunks(psi, u, configs, omegas, events=None):
+    """The sampling loop on the device: for every chunk of samples and every
+    site, W = V . A_i on the contraction engine, then ``qb_sample_select``
+    (two launches per site per chunk).  ``u`` (C x L, fp64), ``configs``
+    (C x L, int64) and ``omegas`` (C, fp64, ones) are contiguous device
+    tensors; returns the number of chunks.  ``events``: a list that receives
+    one (rows, site, start, after-contraction, after-selection) tuple of
+    recorded CUDA events per step (benchmarks)."""
+    import torch
+    from . import _lib
+    C, L = u.shape
+    dt = psi[0].t.dtype
+    row_bytes = max(a.shape[1] * a.shape[2] for a in psi) * psi[0].t.element_size()
+    chunk = max(1, min(C, SAMPLE_CHUNK_BYTES // row_bytes))
+    code = _lib.qb_dtype(dt)
+    lib = _lib.load()
+    n_chunks = 0
+    for c0 in range(0, C, chunk):
+        cc = min(chunk, C - c0)
+        V = torch.ones((cc, 1), dtype=dt, device=u.device)
+        for i, A in enumerate(psi):
+            _, d, r = A.shape
+            if events is not None:
+                ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+                ev[0].record()
+            W = contract_pair(V, [0, 1], A.t, [1, 2, 3], [0, 2, 3], conj_b=A.cj)
+            if events is not None:
+                ev[1].record()
+            V = torch.empty((cc, r), dtype=dt, device=u.device)
+            rc = lib.qb_sample_select(
+                code, cc, d, r, W.data_ptr(), u.data_ptr() + 8 * (c0 * L + i), L,
+                configs.data_ptr() + 8 * (c0 * L + i), L, omegas.data_ptr() + 8 * c0,
+                V.data_ptr(), _lib.stream_ptr())
+            _lib.check(rc, "qb_sample_select")
+            if events is not None:
+                ev[2].record()
+                events.append((cc, i, *ev))
+        n_chunks += 1
+    return n_chunks
+
+
+def mps_sample(sites, C, seed=None):
+    """``C`` configurations drawn from |psi|^2 of an open-boundary MPS, with
+    their probabilities: ``MatrixProductState.sample(C, seed)``
+    (tn1d/core.py:3943-3990) for (l, p, r) device arrays, all samples at once.
+
+    Returns ``(configs, omegas)``: int64 (C, L) and float64 (C,) numpy arrays;
+    ``zip(configs.tolist(), omegas)`` is the reference's sequence of
+    ``(config, omega)``.  The uniforms are ``rng.random((C, L))`` of
+    ``rng = np.random.default_rng(seed)`` (a Generator, or a
+    ``quimb_b200.random.default_rng`` one, is used and advanced by C * L
+    doubles), the very draws the reference makes one ``rng.choice`` at a time,
+    so the configurations agree sample for sample.  Unlike the reference, the
+    selected row is renormalised at every site (no underflow of long chains);
+    the distribution and the probabilities are the same.
+
+    float32 / complex64 states are widened once; the caller's sites are left
+    untouched.  Raises ``ValueError`` when a probability vector is not finite
+    or sums to zero (as ``rng.choice`` does)."""
+    import torch
+    C = int(C)
+    if C < 0:
+        raise ValueError("mps_sample: C must be >= 0")
+    L = len(sites)
+    if C == 0:
+        return np.empty((0, L), dtype=np.int64), np.empty((0,), dtype=np.float64)
+    rng = _sample_rng(seed)
+    psi, nrm = _sample_prepare(sites)
+    dev = psi[0].t.device
+    u = torch.from_numpy(rng.random((C, L))).to(dev)
+    configs = torch.empty((C, L), dtype=torch.int64, device=dev)
+    omegas = torch.ones((C,), dtype=torch.float64, device=dev)
+    _sample_chunks(psi, u, configs, omegas)
+    configs, omegas, nrm = configs.cpu().numpy(), omegas.cpu().numpy(), complex(nrm.item())
+    if not (np.isfinite(nrm) and nrm != 0) or (configs < 0).any():
+        raise ValueError("mps_sample: probabilities contain NaN or sum to zero")
+    return configs, omegas
+
+
+def mps_sample_configuration(sites, seed=None):
+    """One configuration and its probability,
+    ``MatrixProductState.sample_configuration(seed)`` (tn1d/core.py:
+    3871-3941): ``(list of int, float)``, the first draw of
+    :func:`mps_sample` with the same seed."""
+    configs, omegas = mps_sample(sites, 1, seed=seed)
+    return configs[0].tolist(), float(omegas[0])
 
 
 # ------------------------------------------------------ MPS compression etc. ---
