@@ -48,13 +48,13 @@ int gemm_f64(const double *A, int64_t a_rs, int64_t a_cs, const double *B,
   const int32_t la[2] = {0, 1}, lb[2] = {1, 2}, lc[2] = {0, 2};
   PairPlan plan;
   if (!splitk_ws) max_splitk = 1;
-  int rc = plan_pair(&a, la, &b, lb, &c, lc, 0, 0, plan, -1, max_splitk);
+  int rc = plan_pair(&a, la, &b, lb, &c, lc, 0, 0, plan, max_splitk);
   if (rc) return rc;
   plan.streamk = 0;  // internal GEMMs use classic launches (small scratch)
   if (plan.p.splitk > 1) {
     if (plan_scratch_bytes(plan) > splitk_ws_elems * 8) {
       // not enough scratch: redo the plan without split-K
-      rc = plan_pair(&a, la, &b, lb, &c, lc, 0, 0, plan, -1, 1);
+      rc = plan_pair(&a, la, &b, lb, &c, lc, 0, 0, plan, 1);
       if (rc) return rc;
       plan.streamk = 0;
     } else {
@@ -118,15 +118,6 @@ static bool want_stream(int engine, const PairPlan &plan) {
   return engine == QB_ENGINE_STREAM && stream_eligible(plan);
 }
 
-// QB_FORCE_CFG: tuning/debug override of the tile configuration
-static int force_cfg() {
-  static const int v = [] {
-    const char *e = getenv("QB_FORCE_CFG");
-    return e ? atoi(e) : -1;
-  }();
-  return v;
-}
-
 // The one dispatch decision of a pairwise contraction (engine = the low byte
 // of the caller's engine argument).  contract_pair_impl launches what this
 // returns and qb_contract_pair_route reports it.
@@ -183,7 +174,7 @@ int qb_contract_pair_route(const qb_tensor_t *A, const int32_t *la,
                            const qb_tensor_t *C, const int32_t *lc, int engine,
                            int64_t *out) {
   PairPlan plan;
-  int rc = plan_pair(A, la, B, lb, C, lc, 0, 0, plan, force_cfg());
+  int rc = plan_pair(A, la, B, lb, C, lc, 0, 0, plan);
   if (rc) return rc;
   const Route r = select_route(plan, engine & 0xff);
   out[0] = r.kind; out[1] = r.cfg; out[2] = r.splitk; out[3] = r.streamk;
@@ -253,7 +244,7 @@ static int contract_pair_impl(const qb_tensor_t *A, const int32_t *la,
   PairPlan plan;
   const bool ws_zeroed = (engine & QB_ENGINE_WS_ZEROED) != 0;
   engine &= 0xff;
-  int rc = plan_pair(A, la, B, lb, C, lc, conjA, conjB, plan, force_cfg());
+  int rc = plan_pair(A, la, B, lb, C, lc, conjA, conjB, plan);
   if (rc) return rc;
   const Route route = select_route(plan, engine);
   if (route.kind == ROUTE_WIDEN) return check_device_dtype(plan);

@@ -163,7 +163,7 @@ struct SkSeg {
 };
 
 template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
-          bool CPLX, int LA = -1, int LB = -1, int DBG = 0>
+          bool CPLX, int LA = -1, int LB = -1>
 __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
                                               int64_t zb, int ks, int64_t kbeg,
                                               int64_t kend, const SkSeg sk) {
@@ -330,28 +330,22 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
   }
 
   const bool early = ((warp >> 2) & 1) == 0 || (NT <= 128);
-  // DBG (tuning builds only, QB_DBG): 1 no tile loads, 2 no barriers,
-  // 4 fragments read once -- results are garbage, only the timing is used
-  constexpr int dbg = DBG;
   double af[MT][4], bf[NT8][2];
 #pragma unroll 1
   for (int kb = 0; kb < nkb; ++kb) {
-    if (!(dbg & 2)) {
-      cp_async_wait<STAGES - 2>();
-      __syncthreads();  // stage kb landed; stage kb-1 free; next ktab visible
-    }
+    cp_async_wait<STAGES - 2>();
+    __syncthreads();  // stage kb landed; stage kb-1 free; next ktab visible
     if (kb == 0) QB_TRACE(3);
     // the two warps that share a scheduler (warp, warp+4) issue their
     // gathers at different points of the k-block so that one of them always
     // has DMMAs ready while the other does address arithmetic
-    if (early && !(dbg & 1)) issue(kb + STAGES - 1);
+    if (early) issue(kb + STAGES - 1);
     fill_ktab(kb + STAGES);
     const double *tA = sA + (size_t)(kb % STAGES) * Cfg::A_ELEMS;
     const double *tB = sB + (size_t)(kb % STAGES) * Cfg::B_ELEMS;
 #pragma unroll
     for (int kk = 0; kk < BK; kk += 8) {
-      if (kk == 8 && !early && !(dbg & 1)) issue(kb + STAGES - 1);
-      if (!(dbg & 4) || kb == 0) {
+      if (kk == 8 && !early) issue(kb + STAGES - 1);
 #pragma unroll
       for (int i = 0; i < MT; ++i) {
         const int r = wm0 + i * 16 + g;
@@ -371,7 +365,6 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
           bf[j][0] = tB[c * sBn + (kk + t) * sBk];
           bf[j][1] = tB[c * sBn + (kk + t + 4) * sBk];
         }
-      }
       }
 #pragma unroll
       for (int i = 0; i < MT; ++i)
@@ -477,7 +470,7 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
 }
 
 template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
-          bool CPLX, int LA = -1, int LB = -1, int DBG = 0>
+          bool CPLX, int LA = -1, int LB = -1>
 __global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
     contract_f64_kernel(const __grid_constant__ ContractParams p) {
   const int64_t Kh = CPLX ? 2 * p.K : p.K;
@@ -485,7 +478,7 @@ __global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
   const int64_t kbeg = (int64_t)ks * p.k_per_split;  // in real-k units
   const int64_t kend = min(Kh, kbeg + p.k_per_split);
   SkSeg sk{0, (int)(blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z)), 0, 0, nullptr, nullptr, 0};
-  contract_tile<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB, DBG>(
+  contract_tile<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB>(
       p, blockIdx.x, blockIdx.y, ks, kbeg, kend, sk);
 }
 
@@ -574,14 +567,11 @@ __global__ void splitk_reduce_f64_kernel(const __grid_constant__ ContractParams 
 // become resident while the previous kernel in the stream drains (they build
 // their offset tables, then block in griddepcontrol.wait until it has
 // completed and flushed), which hides the launch latency between the
-// back-to-back contractions of a tree / an MPS sweep.
+// back-to-back contractions of a tree / an MPS sweep.  Launches recorded into
+// a stream capture go without the attribute.
 template <typename Kern>
 static int launch_pdl(Kern kern, dim3 grid, int threads, size_t smem, cudaStream_t st,
                       const ContractParams &p) {
-  static const bool pdl = [] {
-    const char *e = getenv("QB_PDL");
-    return e ? atoi(e) != 0 : true;
-  }();
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem;
@@ -589,7 +579,7 @@ static int launch_pdl(Kern kern, dim3 grid, int threads, size_t smem, cudaStream
   cudaLaunchAttribute attr[1];
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   cudaStreamIsCapturing(st, &cap);
-  if (pdl && cap == cudaStreamCaptureStatusNone) {
+  if (cap == cudaStreamCaptureStatusNone) {
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
@@ -600,10 +590,10 @@ static int launch_pdl(Kern kern, dim3 grid, int threads, size_t smem, cudaStream
 }
 
 template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
-          bool CPLX, int LA = -1, int LB = -1, int DBG = 0>
+          bool CPLX, int LA = -1, int LB = -1>
 static int launch_cfg(const ContractParams &p, cudaStream_t st) {
   using Cfg = KernelCfg<BM, BN, BK, WARPS_M, WARPS_N, STAGES>;
-  auto kern = contract_f64_kernel<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB, DBG>;
+  auto kern = contract_f64_kernel<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB>;
   static bool attr_set = false;
   if (!attr_set) {
     QB_CUDA_CHECK(cudaFuncSetAttribute(
@@ -619,12 +609,14 @@ static int launch_cfg(const ContractParams &p, cudaStream_t st) {
   return launch_pdl(kern, grid, Cfg::NT, Cfg::SMEM, st, p);
 }
 
-// the cfg-0 kernels are specialised on the shared-memory layout of real
-// operands (a_kmajor / b_kmajor, plan.h); the route carries the choice
-template <bool CPLX, int LA, int LB, int BK = 16, int STAGES = 4>
+// The cfg-0 (large) tile: 128 x 128, BK 32, 3 stages, 8 warps.  Its real
+// kernels are specialised on the shared-memory layout of the operands
+// (a_kmajor / b_kmajor, plan.h); the route carries the choice.  The complex
+// kernel takes its layout at run time.
+template <bool CPLX, int LA, int LB>
 static int launch_streamk_l(const PairPlan &plan, cudaStream_t st) {
-  using Cfg = KernelCfg<128, 128, BK, 2, 4, STAGES>;
-  auto kern = contract_f64_streamk_kernel<128, 128, BK, 2, 4, STAGES, CPLX, LA, LB>;
+  using Cfg = KernelCfg<128, 128, 32, 2, 4, 3>;
+  auto kern = contract_f64_streamk_kernel<128, 128, 32, 2, 4, 3, CPLX, LA, LB>;
   static bool attr_set = false;
   if (!attr_set) {
     QB_CUDA_CHECK(cudaFuncSetAttribute(
@@ -639,41 +631,30 @@ static int launch_streamk_l(const PairPlan &plan, cudaStream_t st) {
 
 template <bool CPLX>
 static int launch_streamk(const PairPlan &plan, const Route &r, cudaStream_t st) {
-  const bool bk32 = r.bk == 32;
-  if (!CPLX && r.layout >= 0) {
-    switch (r.layout + (bk32 ? 4 : 0)) {
+  if constexpr (CPLX) {
+    return launch_streamk_l<true, -1, -1>(plan, st);
+  } else {
+    switch (r.layout) {
       case 0: return launch_streamk_l<false, 0, 0>(plan, st);
       case 1: return launch_streamk_l<false, 0, 1>(plan, st);
       case 2: return launch_streamk_l<false, 1, 0>(plan, st);
-      case 3: return launch_streamk_l<false, 1, 1>(plan, st);
-      case 4: return launch_streamk_l<false, 0, 0, 32, 3>(plan, st);
-      case 5: return launch_streamk_l<false, 0, 1, 32, 3>(plan, st);
-      case 6: return launch_streamk_l<false, 1, 0, 32, 3>(plan, st);
-      default: return launch_streamk_l<false, 1, 1, 32, 3>(plan, st);
+      default: return launch_streamk_l<false, 1, 1>(plan, st);
     }
   }
-  if (bk32) return launch_streamk_l<CPLX, -1, -1, 32, 3>(plan, st);
-  return launch_streamk_l<CPLX, -1, -1>(plan, st);
 }
 
 template <bool CPLX>
 static int launch_cfg0(const ContractParams &p, const Route &r, cudaStream_t st) {
-  if (!CPLX) {
-    if (r.layout >= 0) {
-      switch (r.layout + (r.bk == 32 ? 4 : 0)) {
-        case 0: return launch_cfg<128, 128, 16, 2, 4, 4, false, 0, 0>(p, st);
-        case 1: return launch_cfg<128, 128, 16, 2, 4, 4, false, 0, 1>(p, st);
-        case 2: return launch_cfg<128, 128, 16, 2, 4, 4, false, 1, 0>(p, st);
-        case 3: return launch_cfg<128, 128, 16, 2, 4, 4, false, 1, 1>(p, st);
-        case 4: return launch_cfg<128, 128, 32, 2, 4, 3, false, 0, 0>(p, st);
-        case 5: return launch_cfg<128, 128, 32, 2, 4, 3, false, 0, 1>(p, st);
-        case 6: return launch_cfg<128, 128, 32, 2, 4, 3, false, 1, 0>(p, st);
-        default: return launch_cfg<128, 128, 32, 2, 4, 3, false, 1, 1>(p, st);
-      }
+  if constexpr (CPLX) {
+    return launch_cfg<128, 128, 32, 2, 4, 3, true>(p, st);
+  } else {
+    switch (r.layout) {
+      case 0: return launch_cfg<128, 128, 32, 2, 4, 3, false, 0, 0>(p, st);
+      case 1: return launch_cfg<128, 128, 32, 2, 4, 3, false, 0, 1>(p, st);
+      case 2: return launch_cfg<128, 128, 32, 2, 4, 3, false, 1, 0>(p, st);
+      default: return launch_cfg<128, 128, 32, 2, 4, 3, false, 1, 1>(p, st);
     }
   }
-  if (r.bk == 32) return launch_cfg<128, 128, 32, 2, 4, 3, CPLX>(p, st);
-  return launch_cfg<128, 128, 16, 2, 4, 4, CPLX>(p, st);
 }
 
 template <bool CPLX>

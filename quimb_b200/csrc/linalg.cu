@@ -8,23 +8,14 @@
 //                  the formation of Q are GEMMs on the contraction kernel.
 //                  The stabilisation (diag(R) >= 0, phase into Q) is a fused
 //                  epilogue kernel.
-//   qb_svd      <- the LAPACK gesdd call inside svd_truncated
-//                  (decomp.py:1032-1055): one-sided block Jacobi on the
-//                  R factor of a QR preconditioner.  Per round, one CTA per
-//                  column-block pair: Gram matrix with DMMA-free register
-//                  tiles, cyclic Jacobi eigen-solve of the 2b x 2b Gram in
-//                  shared memory, rotation applied to the columns of the
-//                  working matrix and of V.  The working set (n x n twice)
-//                  is 64 MB at n = 2048 (the H100's L2 holds 50 MB).
 //   qb_svals_to_keep <- _compute_number_svals_to_keep_numba + renorm factor
 //                  (decomp.py:901-965), host side, bit-for-bit the same
 //                  summation order as the reference.
+// The SVD (qb_svd, qb_svd_trunc) is in svd_jacobi.cu.
 #include <cooperative_groups.h>
 #include <math.h>
-#include <stdlib.h>
 
 #include <algorithm>
-#include <vector>
 
 #include "internal.h"
 
@@ -640,574 +631,3 @@ int qb_svals_to_keep(const double *s, int64_t n, double cutoff,
 }
 
 }  // extern "C"
-
-// =========================================================================
-//                      one-sided block Jacobi SVD
-// =========================================================================
-namespace qb {
-
-constexpr int JB = 16;          // columns per block
-constexpr int JP = 2 * JB;      // columns per pair
-constexpr int JCH = 64;         // rows per streamed chunk
-constexpr int JPITCH = JP + 4;  // smem pitch (== 4 mod 16 doubles)
-
-struct JacobiParams {
-  double *W;       // rows_w x ld  working matrix (columns get orthogonalised)
-  double *V;       // rows_v x ld  accumulated right rotations
-  int64_t ld;
-  int rows_w, rows_v;
-  int nblk;        // number of column blocks (even)
-  int round;       // 0 .. nblk-2
-  double tol;
-  int *flag;       // set to 1 when any pair still needed rotating
-  int inner_max;   // max inner Jacobi sweeps per visit
-  unsigned long long *trace;  // tuning (QB_TRACE): phase stamps of cluster 0
-  int trace_slot;             // ring of 1024 rounds
-};
-
-__device__ __forceinline__ unsigned long long jac_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-#define JAC_TRACE(ph)                                                     \
-  do {                                                                    \
-    if (P.trace && blockIdx.x == 0 && threadIdx.x == 0)                   \
-      P.trace[(size_t)P.trace_slot * 8 + (ph)] = jac_ns();             \
-  } while (0)
-
-__device__ __forceinline__ void rr_pair(int k, int round, int nblk, int &p, int &q) {
-  // circle-method round robin over nblk players
-  const int m = nblk - 1;
-  int a, b;
-  if (k == 0) { a = m; b = round; }
-  else { a = (round + k) % m; b = (round - k + m) % m; }
-  p = min(a, b); q = max(a, b);
-}
-
-__device__ __forceinline__ void jac_load_chunk(double (*Xs)[JPITCH], const double *M,
-                                               int64_t ld, int rows, int row0,
-                                               int cp, int cq, int tid) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int idx = tid + 256 * i;       // 1024 double2 per chunk
-    const int r = idx >> 4, c2 = (idx & 15) * 2;
-    const int gc = (c2 < JB) ? (cp + c2) : (cq + c2 - JB);
-    const int gr = row0 + r;
-    const bool ok = gr < rows;
-    const double *src = ok ? (M + (int64_t)gr * ld + gc) : M;
-    cp_async16(smem_u32(&Xs[r][c2]), src, ok ? 16 : 0);
-  }
-}
-
-constexpr int JCSZ = 2;         // CTAs (one cluster) per column-block pair
-
-// One round-robin round of the one-sided block Jacobi method.  A CLUSTER of
-// JCSZ CTAs owns one pair of column blocks (2 x 16 columns); the rows of W
-// and V are dealt round-robin (64-row chunks) to the CTAs of the cluster:
-//   1. partial Gram of the 32 columns by DMMA from a 4-stage cp.async stream,
-//      reduced over warps and then over the cluster through distributed
-//      shared memory (fixed order: deterministic);
-//   2. every CTA diagonalises the same 32 x 32 Gram by parallel-ordered
-//      cyclic Jacobi (two-sided rotations fused into one pass over a
-//      ping-pong copy of the Gram: one barrier per step), sorted descending;
-//   3. the rotation is applied by DMMA to this CTA's rows of W and of V.
-template <int JSTG>  // cp.async stages of the row-chunk stream
-__global__ void __cluster_dims__(JCSZ, 1, 1) __launch_bounds__(256)
-    jacobi_pair_kernel(const JacobiParams P) {
-  namespace cg = cooperative_groups;
-  cg::cluster_group cluster = cg::this_cluster();
-  const int rank = (int)cluster.block_rank();
-  extern __shared__ __align__(16) unsigned char jac_smem[];
-  double(*Xs)[JCH][JPITCH] = reinterpret_cast<double(*)[JCH][JPITCH]>(jac_smem);
-  __shared__ double Gbuf[2][JP][JP + 1];
-  double(*G)[JP + 1] = Gbuf[0];   // current Gram; the eigen-solve ping-pongs
-  double(*Gn)[JP + 1] = Gbuf[1];
-  __shared__ double Gpart[JP][JP];
-  __shared__ __align__(16) double Jm[JP][JPITCH];
-  __shared__ double redmax[8];
-  __shared__ int rank_s[JP];
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int g = lane >> 2, t = lane & 3;
-  int bp, bq;
-  rr_pair(blockIdx.x / JCSZ, P.round, P.nblk, bp, bq);
-  const int cp = bp * JB, cq = bq * JB;
-
-  JAC_TRACE(0);
-  // ---------------- phase 1: partial Gram over this CTA's row chunks --------
-  double acc[2][4][4];
-#pragma unroll
-  for (int i = 0; i < 2; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-#pragma unroll
-      for (int v = 0; v < 4; ++v) acc[i][j][v] = 0.0;
-  {
-    const int nch_all = (P.rows_w + JCH - 1) / JCH;
-    const int nmine = (nch_all - rank + JCSZ - 1) / JCSZ;  // chunks rank, rank+JCSZ, ...
-    auto issue = [&](int i) {
-      if (i < nmine)
-        jac_load_chunk(Xs[i % JSTG], P.W, P.ld, P.rows_w, (rank + i * JCSZ) * JCH, cp, cq, tid);
-      cp_async_commit();
-    };
-    for (int s = 0; s < JSTG - 1; ++s) issue(s);
-    for (int i = 0; i < nmine; ++i) {
-      cp_async_wait<JSTG - 2>();
-      __syncthreads();
-      issue(i + JSTG - 1);
-      const double(*X)[JPITCH] = Xs[i % JSTG];
-      const int kb = warp * 8;
-      double af[2][4], bf[4][2];
-#pragma unroll
-      for (int a = 0; a < 2; ++a) {
-        af[a][0] = X[kb + t][a * 16 + g];
-        af[a][1] = X[kb + t][a * 16 + g + 8];
-        af[a][2] = X[kb + t + 4][a * 16 + g];
-        af[a][3] = X[kb + t + 4][a * 16 + g + 8];
-      }
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        bf[j][0] = X[kb + t][j * 8 + g];
-        bf[j][1] = X[kb + t + 4][j * 8 + g];
-      }
-      // the Gram is symmetric: the lower-left 16 x 16 block (a = 1, j < 2)
-      // is the mirror of the upper-right one and is not computed
-#pragma unroll
-      for (int a = 0; a < 2; ++a)
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (a == 0 || j >= 2) dmma_16x8x8(acc[a][j], af[a], bf[j]);
-    }
-    cp_async_wait<0>();
-    __syncthreads();
-  }
-  JAC_TRACE(1);
-  // deterministic reduction over the 8 warps into Gpart: every warp parks its
-  // fragment in the (now idle) stream buffers, one barrier, then each thread
-  // sums four entries over the warps in a fixed order
-  {
-    double *scr = &Xs[0][0][0];  // 8 x 32 x 32 doubles <= JSTG * JCH * JPITCH
-#pragma unroll
-    for (int i = 0; i < 2; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = i * 16 + g + h * 8, c = j * 8 + 2 * t;
-          *reinterpret_cast<double2 *>(&scr[(warp * JP + r) * JP + c]) =
-              make_double2(acc[i][j][2 * h], acc[i][j][2 * h + 1]);
-        }
-    __syncthreads();
-    for (int idx = tid; idx < JP * JP; idx += 256) {
-      const int r = idx / JP, c = idx % JP;
-      const int src = (r >= 16 && c < 16) ? (c * JP + r) : idx;  // mirrored block
-      double sum = 0.0;
-#pragma unroll
-      for (int w = 0; w < 8; ++w) sum += scr[w * JP * JP + src];
-      Gpart[r][c] = sum;
-    }
-  }
-  cluster.sync();
-  // full Gram = sum over the cluster (same order everywhere), symmetrised
-  for (int idx = tid; idx < JP * JP; idx += 256) {
-    const int r = idx / JP, c = idx % JP;
-    double s = 0.0;
-#pragma unroll
-    for (int q = 0; q < JCSZ; ++q) {
-      const double *gp = cluster.map_shared_rank(&Gpart[0][0], q);
-      s += 0.5 * (gp[r * JP + c] + gp[c * JP + r]);
-    }
-    G[r][c] = s;
-    Jm[r][c] = (r == c) ? 1.0 : 0.0;
-  }
-  __syncthreads();
-  auto offmax = [&]() -> double {
-    double mx = 0.0;
-    for (int idx = tid; idx < JP * JP; idx += 256) {
-      const int r = idx / JP, c = idx % JP;
-      if (r < c) {
-        const double d = G[r][r] * G[c][c];
-        const double v = fabs(G[r][c]);
-        if (d > 0.0) mx = fmax(mx, v / sqrt(d));
-        else if (v > 0.0) mx = fmax(mx, 1.0);
-      }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    if (lane == 0) redmax[warp] = mx;
-    __syncthreads();
-    double m2 = 0.0;
-    for (int w = 0; w < 8; ++w) m2 = fmax(m2, redmax[w]);
-    __syncthreads();
-    return m2;
-  };
-  const double off0 = offmax();
-  JAC_TRACE(2);
-  // all CTAs of the cluster take the same decision (same G)
-  if (off0 <= P.tol) {
-    cluster.sync();  // peers may still be reading our Gpart
-    return;
-  }
-  if (tid == 0 && rank == 0) atomicOr(P.flag, 1);
-
-  // ---------------- phase 2: J^T G J = diag by cyclic Jacobi ----------------
-  // inner sweeps: stop at round-off, or once this visit has reduced the
-  // pair's off-diagonal mass by 1e-4 (at most 3 sweeps): block Jacobi
-  // converges with inexact inner solves, and near convergence one sweep is
-  // enough to reach round-off (quadratic convergence)
-  for (int sweep = 0; sweep < P.inner_max; ++sweep) {
-    if (sweep > 0) {
-      const double off = offmax();
-      if (off <= 1e-15 || off <= 1e-4 * off0) break;
-    }
-    for (int step = 0; step < JP - 1; ++step) {
-      // One barrier per step: thread (k1, k2) owns the 2x2 block (rows of pair
-      // k1) x (columns of pair k2).  The 16 rotations of the step are computed
-      // once per warp (lanes 0-15, pinned arithmetic so that all warps get
-      // bit-identical c, s) and handed out by shuffles; the rotated block goes
-      // to the other Gram buffer; J <- J R for column pair k2, rows k1, k1+16.
-      const int k1 = tid >> 4, k2 = tid & 15;
-      int p1, q1, p2, q2;
-      rr_pair(k1, step, JP, p1, q1);
-      rr_pair(k2, step, JP, p2, q2);
-      double c = 1.0, s = 0.0;
-      if (lane < 16) {  // lane == k2 here
-        const double app = G[p2][p2], aqq = G[q2][q2], apq = G[p2][q2];
-        if (fabs(apq) > 1e-300) {
-          // t = sgn(z) / (|z| + sqrt(1 + z^2)), z = (aqq - app) / (2 apq)
-          const double a = __dsub_rn(aqq, app), b = __dmul_rn(2.0, apq);
-          const double h = sqrt(__fma_rn(a, a, __dmul_rn(b, b)));
-          const double tt = __ddiv_rn(copysign(fabs(b), __dmul_rn(a, b)), __dadd_rn(fabs(a), h));
-          c = rsqrt(__fma_rn(tt, tt, 1.0));
-          s = __dmul_rn(c, tt);
-        }
-      }
-      const double c2 = __shfl_sync(0xffffffffu, c, k2), s2 = __shfl_sync(0xffffffffu, s, k2);
-      const double c1 = __shfl_sync(0xffffffffu, c, k1), s1 = __shfl_sync(0xffffffffu, s, k1);
-      {
-        const double gpp = G[p1][p2], gpq = G[p1][q2], gqp = G[q1][p2], gqq = G[q1][q2];
-        // columns first
-        const double a0 = c2 * gpp - s2 * gpq, a1 = s2 * gpp + c2 * gpq;
-        const double b0 = c2 * gqp - s2 * gqq, b1 = s2 * gqp + c2 * gqq;
-        // then rows
-        double n00 = c1 * a0 - s1 * b0, n01 = c1 * a1 - s1 * b1;
-        double n10 = s1 * a0 + c1 * b0, n11 = s1 * a1 + c1 * b1;
-        if (k1 == k2) { n01 = 0.0; n10 = 0.0; }  // the annihilated pair
-        Gn[p1][p2] = n00; Gn[p1][q2] = n01; Gn[q1][p2] = n10; Gn[q1][q2] = n11;
-#pragma unroll
-        for (int it = 0; it < 2; ++it) {
-          const int r = k1 + 16 * it;
-          const double jp = Jm[r][p2], jq = Jm[r][q2];
-          Jm[r][p2] = c2 * jp - s2 * jq;
-          Jm[r][q2] = s2 * jp + c2 * jq;
-        }
-      }
-      __syncthreads();
-      { double(*tmp)[JP + 1] = G; G = Gn; Gn = tmp; }
-    }
-  }
-  JAC_TRACE(3);
-  // sort: larger column norms first (ties by index) -> new column order
-  if (tid < JP) {
-    const double d = G[tid][tid];
-    int rk = 0;
-    for (int j = 0; j < JP; ++j) {
-      const double dj = G[j][j];
-      rk += (dj > d) || (dj == d && j < tid);
-    }
-    rank_s[tid] = rk;
-  }
-  __syncthreads();
-  for (int idx = tid; idx < JP * JP; idx += 256) {
-    const int r = idx / JP, c = idx % JP;
-    G[r][rank_s[c]] = Jm[r][c];
-  }
-  __syncthreads();
-  for (int idx = tid; idx < JP * JP; idx += 256) {
-    const int r = idx / JP, c = idx % JP;
-    Jm[r][c] = G[r][c];
-  }
-  __syncthreads();
-
-  JAC_TRACE(4);
-  // ---------------- phase 3: apply J to this CTA's rows of W and V ----------
-  {
-    const int nchw = (P.rows_w + JCH - 1) / JCH, nchv = (P.rows_v + JCH - 1) / JCH;
-    const int ntot = nchw + nchv;
-    const int nmine = (ntot - rank + JCSZ - 1) / JCSZ;
-    auto chunk_src = [&](int i, double *&M, int &rows, int &row0) {
-      const int ch = rank + i * JCSZ;
-      if (ch < nchw) { M = P.W; rows = P.rows_w; row0 = ch * JCH; }
-      else { M = P.V; rows = P.rows_v; row0 = (ch - nchw) * JCH; }
-    };
-    auto issue = [&](int i) {
-      if (i < nmine) {
-        double *M; int rows, row0;
-        chunk_src(i, M, rows, row0);
-        jac_load_chunk(Xs[i % JSTG], M, P.ld, rows, row0, cp, cq, tid);
-      }
-      cp_async_commit();
-    };
-    for (int s = 0; s < JSTG - 1; ++s) issue(s);
-    const int mt = warp & 3, nh = warp >> 2;  // 16 rows x 16 cols per warp
-    for (int i = 0; i < nmine; ++i) {
-      cp_async_wait<JSTG - 2>();
-      __syncthreads();
-      issue(i + JSTG - 1);
-      double *M; int rows, row0;
-      chunk_src(i, M, rows, row0);
-      const double(*X)[JPITCH] = Xs[i % JSTG];
-      double c2[2][4];
-#pragma unroll
-      for (int j = 0; j < 2; ++j)
-#pragma unroll
-        for (int v = 0; v < 4; ++v) c2[j][v] = 0.0;
-#pragma unroll
-      for (int kk = 0; kk < JP; kk += 8) {
-        double af[4], bf[2][2];
-        af[0] = X[mt * 16 + g][kk + t];
-        af[1] = X[mt * 16 + g + 8][kk + t];
-        af[2] = X[mt * 16 + g][kk + t + 4];
-        af[3] = X[mt * 16 + g + 8][kk + t + 4];
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          bf[j][0] = Jm[kk + t][nh * 16 + j * 8 + g];
-          bf[j][1] = Jm[kk + t + 4][nh * 16 + j * 8 + g];
-        }
-#pragma unroll
-        for (int j = 0; j < 2; ++j) dmma_16x8x8(c2[j], af, bf[j]);
-      }
-#pragma unroll
-      for (int j = 0; j < 2; ++j)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = row0 + mt * 16 + g + h * 8;
-          const int c = nh * 16 + j * 8 + 2 * t;  // column within the pair
-          if (r < rows) {
-            const int gc = (c < JB) ? (cp + c) : (cq + c - JB);
-            *reinterpret_cast<double2 *>(M + (int64_t)r * P.ld + gc) =
-                make_double2(c2[j][2 * h], c2[j][2 * h + 1]);
-          }
-        }
-    }
-    cp_async_wait<0>();
-  }
-  JAC_TRACE(5);
-  cluster.sync();  // nobody exits while peers may read its shared memory
-  JAC_TRACE(6);
-}
-
-// column norms of W (rows x ld, first ncols columns)
-__global__ void __launch_bounds__(256)
-    colnorm_kernel(const double *__restrict__ W, int64_t ld, int rows, int ncols,
-                   double *__restrict__ out) {
-  // one warp per 32 columns chunk-row: simple and coalesced: block handles
-  // 32 columns, threads (32 x 8) walk rows
-  __shared__ double sh[8][33];
-  const int c = blockIdx.x * 32 + (threadIdx.x & 31);
-  const int ry = threadIdx.x >> 5;
-  double s = 0.0;
-  if (c < ncols)
-    for (int r = ry; r < rows; r += 8) {
-      const double v = W[(int64_t)r * ld + c];
-      s += v * v;
-    }
-  sh[ry][threadIdx.x & 31] = s;
-  __syncthreads();
-  if (ry == 0 && c < ncols) {
-    double tot = 0.0;
-    for (int k = 0; k < 8; ++k) tot += sh[k][threadIdx.x & 31];
-    out[c] = sqrt(tot);
-  }
-}
-
-// U_R[:, k] = W[:, perm[k]] / s[perm[k]]   (n x nk, row-major), and
-// VH[k, :] = V[:, perm[k]]^T  (nk x ncols_v rows of V)
-__global__ void __launch_bounds__(256)
-    svd_gather_kernel(const double *__restrict__ W, const double *__restrict__ V,
-                      int64_t ld, int rows_w, int rows_v, int nk,
-                      const int *__restrict__ perm, const double *__restrict__ s,
-                      double *__restrict__ UR, double *__restrict__ VH) {
-  const int64_t tot_u = (int64_t)rows_w * nk, tot_v = (int64_t)nk * rows_v;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < tot_u + tot_v;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    if (i < tot_u) {
-      const int64_t r = i / nk;
-      const int k = (int)(i - r * nk);
-      const int c = perm[k];
-      // W = R^T was orthogonalised: R = Z S Y^T with Z the accumulated
-      // rotations (-> U_R) and Y the normalised columns of W (-> V)
-      UR[i] = V[r * ld + c];
-    } else {
-      const int64_t j = i - tot_u;
-      const int k = (int)(j / rows_v);
-      const int64_t r = j - (int64_t)k * rows_v;
-      const int c = perm[k];
-      const double sv = s[c];
-      VH[j] = (sv > 0.0) ? W[r * ld + c] / sv : 0.0;
-    }
-  }
-}
-
-__global__ void pad_copy_kernel(const double *__restrict__ src, int64_t rows,
-                                int64_t cols, int64_t ld_src, double *__restrict__ dst,
-                                int64_t ld_dst, int64_t rows_dst, int identity) {
-  // dst (rows_dst x ld_dst) = [src | 0] (or the identity when src == null)
-  const int64_t tot = rows_dst * ld_dst;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < tot;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t r = i / ld_dst, c = i - r * ld_dst;
-    double v = 0.0;
-    if (identity == 1) v = (r == c) ? 1.0 : 0.0;
-    else if (r < rows && c < cols)
-      v = (identity == 2) ? src[c * ld_src + r] : src[r * ld_src + c];  // 2: transposed
-    dst[i] = v;
-  }
-}
-
-struct SvdGeom {
-  int64_t npad, qr_off, q1_off, r_off, w_off, v_off, s_off, ur_off, perm_off,
-      flag_off, xt_off, total;
-};
-
-static bool svd_geometry(int64_t m, int64_t n, SvdGeom &g) {
-  // m >= n here
-  QrGeom q;
-  if (!qr_geometry(m, n, q)) return false;
-  g.npad = ((n + JP - 1) / JP) * JP;
-  auto al = [](int64_t x) { return (x + 31) / 32 * 32; };  // 256-byte sections
-  int64_t off = 0;
-  g.qr_off = off; off += al(q.total);
-  g.q1_off = off; off += al(m * n);
-  g.r_off = off; off += al(n * n);
-  g.w_off = off; off += al(n * g.npad);
-  g.v_off = off; off += al(g.npad * g.npad);
-  g.s_off = off; off += al(g.npad);
-  g.ur_off = off; off += al(n * n);
-  g.perm_off = off; off += al((g.npad + 1) / 2 + 1);   // ints
-  g.flag_off = off; off += 32;
-  g.xt_off = off; off += 0;
-  g.total = off;
-  return true;
-}
-
-// SVD of row-major X (m x n), m >= n.  U (m x n), S (n), VH (n x n).
-int svd_tall_f64_v1(int64_t m, int64_t n, const double *X, double *U,
-                        double *S, double *VH, double *ws, int *sweeps_out,
-                        cudaStream_t st) {
-  SvdGeom g;
-  if (!svd_geometry(m, n, g)) {
-    set_error("qb_svd: unsupported shape %lld x %lld", (long long)m, (long long)n);
-    return -2;
-  }
-  double *Q1 = ws + g.q1_off, *R = ws + g.r_off, *W = ws + g.w_off;
-  double *V = ws + g.v_off, *sv = ws + g.s_off, *UR = ws + g.ur_off;
-  int *perm = reinterpret_cast<int *>(ws + g.perm_off);
-  int *flag = reinterpret_cast<int *>(ws + g.flag_off);
-  const int blocks = sm_count() * 4;
-  int rc = qr_f64(m, n, X, Q1, R, /*stabilized=*/0, ws + g.qr_off, st);
-  if (rc) return rc;
-  const int64_t npad = g.npad;
-  pad_copy_kernel<<<blocks, 256, 0, st>>>(R, n, n, n, W, npad, n, 2);  // W = R^T
-  QB_LAUNCH_CHECK();
-  pad_copy_kernel<<<blocks, 256, 0, st>>>(nullptr, 0, 0, 0, V, npad, npad, 1);
-  QB_LAUNCH_CHECK();
-  // stream depth (QB_JAC_STAGES: 4, 8 or 10): measured identical -- the row
-  // streams are bound by the DMMA rate (64 rows x 32 x 32 FMAs per chunk =
-  // 1024 pipe clocks per SM), not by bytes in flight
-  static const int jstg = [] {
-    const char *e = getenv("QB_JAC_STAGES");
-    const int v = e ? atoi(e) : 4;
-    return v <= 4 ? 4 : (v <= 8 ? 8 : 10);
-  }();
-  const int kJacSmem = jstg * JCH * JPITCH * 8;
-  static bool attr_set = false;
-  if (!attr_set) {
-    QB_CUDA_CHECK(cudaFuncSetAttribute(jacobi_pair_kernel<4>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       4 * JCH * JPITCH * 8));
-    QB_CUDA_CHECK(cudaFuncSetAttribute(jacobi_pair_kernel<8>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       8 * JCH * JPITCH * 8));
-    QB_CUDA_CHECK(cudaFuncSetAttribute(jacobi_pair_kernel<10>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       10 * JCH * JPITCH * 8));
-    attr_set = true;
-  }
-  JacobiParams P;
-  P.W = W; P.V = V; P.ld = npad; P.rows_w = (int)n; P.rows_v = (int)npad;
-  P.nblk = (int)(npad / JB);
-  P.tol = 1e-15 * sqrt((double)n) * 8.0;
-  P.flag = flag;
-  P.trace = trace_buffer() ? trace_buffer() + 16 * 8192 : nullptr;
-  {
-    static const int inner = [] { const char *e = getenv("QB_JAC_INNER"); return e ? atoi(e) : 1; }();
-    P.inner_max = inner;
-  }
-  int sweeps = 0;
-  const int max_sweeps = 60;
-  const int inner0 = P.inner_max;
-  for (; sweeps < max_sweeps; ++sweeps) {
-    // one inner sweep per visit is fastest; fall back to fuller inner solves
-    // if the outer iteration is unusually slow
-    P.inner_max = (sweeps < 25) ? inner0 : std::max(inner0, 4);
-    QB_CUDA_CHECK(cudaMemsetAsync(flag, 0, sizeof(int), st));
-    for (int r = 0; r < P.nblk - 1; ++r) {
-      P.round = r;
-      P.trace_slot = (sweeps * (P.nblk - 1) + r) & 1023;
-      const unsigned grid = (unsigned)(P.nblk / 2) * JCSZ;
-      if (jstg == 4) jacobi_pair_kernel<4><<<grid, 256, kJacSmem, st>>>(P);
-      else if (jstg == 8) jacobi_pair_kernel<8><<<grid, 256, kJacSmem, st>>>(P);
-      else jacobi_pair_kernel<10><<<grid, 256, kJacSmem, st>>>(P);
-      QB_LAUNCH_CHECK();
-    }
-    int h = 0;
-    QB_CUDA_CHECK(cudaMemcpyAsync(&h, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
-    QB_CUDA_CHECK(cudaStreamSynchronize(st));
-    if (!h) break;
-  }
-  if (sweeps_out) *sweeps_out = sweeps;
-  if (sweeps >= max_sweeps) {
-    set_error("qb_svd: Jacobi did not converge in %d sweeps", max_sweeps);
-    return 2;
-  }
-  colnorm_kernel<<<(unsigned)(npad / 32), 256, 0, st>>>(W, npad, (int)n, (int)npad, sv);
-  QB_LAUNCH_CHECK();
-  std::vector<double> hs(npad);
-  QB_CUDA_CHECK(cudaMemcpyAsync(hs.data(), sv, sizeof(double) * npad,
-                                cudaMemcpyDeviceToHost, st));
-  QB_CUDA_CHECK(cudaStreamSynchronize(st));
-  std::vector<int> hp(npad);
-  for (int i = 0; i < npad; ++i) hp[i] = i;
-  std::stable_sort(hp.begin(), hp.end(), [&](int a, int b) {
-    const bool pa = a >= n, pb = b >= n;  // padding columns last
-    if (pa != pb) return pb;
-    return hs[a] > hs[b];
-  });
-  QB_CUDA_CHECK(cudaMemcpyAsync(perm, hp.data(), sizeof(int) * n,
-                                cudaMemcpyHostToDevice, st));
-  // sorted singular values
-  std::vector<double> ss(n);
-  for (int i = 0; i < n; ++i) ss[i] = hs[hp[i]];
-  if (S) QB_CUDA_CHECK(cudaMemcpyAsync(S, ss.data(), sizeof(double) * n,
-                                       cudaMemcpyHostToDevice, st));
-  // U_R, VH (VH rows: the first n rows of V only -- the rest is padding)
-  svd_gather_kernel<<<blocks, 256, 0, st>>>(W, V, npad, (int)n, (int)n, (int)n,
-                                            perm, sv, UR, VH ? VH : UR);
-  QB_LAUNCH_CHECK();
-  QB_CUDA_CHECK(cudaStreamSynchronize(st));  // host vectors go out of scope
-  if (U) {
-    rc = gemm_f64(Q1, n, 1, UR, n, 1, U, n, 1, m, n, n, 1.0, 0.0, st);
-    if (rc) return rc;
-  }
-  return 0;
-}
-
-int64_t svd_v1_workspace_doubles(int64_t m, int64_t n) {
-  SvdGeom g;
-  if (!svd_geometry(m, n, g)) return -1;
-  return g.total;
-}
-
-}  // namespace qb

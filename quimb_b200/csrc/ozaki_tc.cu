@@ -614,19 +614,9 @@ struct OzGeom {
   int64_t off_rmA, off_rmB, off_scA, off_scB, off_slA, off_slB, total;  // bytes
 };
 
-static int oz_slices(bool single) {
-  static int s8 = [] {
-    const char *e = getenv("QB_OZAKI_SLICES");
-    int v = e ? atoi(e) : 8;
-    return std::max(2, std::min(v, OZ_MAXS));
-  }();
-  static int s4 = [] {
-    const char *e = getenv("QB_OZAKI_SLICES_SINGLE");
-    int v = e ? atoi(e) : 4;
-    return std::max(2, std::min(v, OZ_MAXS_SINGLE));
-  }();
-  return single ? s4 : s8;
-}
+// int8 slices per operand: all the accumulator columns the GEMM kernel holds
+// (8 for fp64 / complex128, 4 for fp32 / complex64)
+static int oz_slices(bool single) { return single ? OZ_MAXS_SINGLE : OZ_MAXS; }
 
 static void oz_geometry(const PairPlan &plan, OzGeom &g) {
   const ContractParams &p = plan.p;

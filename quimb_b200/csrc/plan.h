@@ -108,7 +108,7 @@ struct TileCfg {
   int bm, bn, bk, threads;
 };
 static const TileCfg kTileCfgs[] = {
-    {128, 128, 16, 256},  // 0: large
+    {128, 128, 32, 256},  // 0: large (3 stages)
     {64, 64, 16, 128},    // 1: medium
     {128, 32, 16, 128},   // 2: tall (small N)
     {32, 128, 16, 128},   // 3: wide (small M)
@@ -120,30 +120,13 @@ constexpr int kNumTileCfgs = 5;
 // clock at the 1.98 GHz boost clock (data sheet: 67 TFLOP/s over 132 SMs)
 constexpr double kDmmaFmaPerSmUs = 128.0 * 1980.0;
 
-// k-depth of the large tile: 32 (3 stages) or 16 (4 stages); QB_CFG0_BK
-// overrides for tuning
-inline int cfg0_bk() {
-  static const int v = [] {
-    const char *e = getenv("QB_CFG0_BK");
-    int b = e ? atoi(e) : 32;
-    return (b == 16) ? 16 : 32;
-  }();
-  return v;
-}
-inline TileCfg tile_cfg(int c) {
-  TileCfg t = kTileCfgs[c];
-  if (c == 0) t.bk = cfg0_bk();
-  return t;
-}
-
 inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 // returns 0 or a negative argument-error code; fills plan
 inline int plan_pair(const qb_tensor_t *A, const int32_t *la,
                      const qb_tensor_t *B, const int32_t *lb,
                      const qb_tensor_t *C, const int32_t *lc, int conjA,
-                     int conjB, PairPlan &plan, int force_cfg = -1,
-                     int max_splitk = 64) {
+                     int conjB, PairPlan &plan, int max_splitk = 64) {
   if (!A) return -1;
   if (!B) return -3;
   if (!C) return -5;
@@ -339,8 +322,7 @@ inline int plan_pair(const qb_tensor_t *A, const int32_t *la,
   int best_cfg = 1, best_split = 1;
   int64_t best_kper = 0;
   for (int c = 0; c < kNumTileCfgs; ++c) {
-    if (force_cfg >= 0 && force_cfg < kNumTileCfgs && c != force_cfg) continue;
-    const TileCfg tc = tile_cfg(c);
+    const TileCfg &tc = kTileCfgs[c];
     const int64_t tiles = cdiv(M, tc.bm) * cdiv(N, tc.bn) * p.nbatch;
     const int64_t kblocks = std::max<int64_t>(cdiv(Kh, tc.bk), 1);
     const int64_t slots = (int64_t)nsm * kOcc[c];
@@ -368,7 +350,7 @@ inline int plan_pair(const qb_tensor_t *A, const int32_t *la,
   }
   cfg = best_cfg;
   plan.cfg = cfg;
-  const TileCfg tc = tile_cfg(cfg);
+  const TileCfg &tc = kTileCfgs[cfg];
   p.tiles_m = (int32_t)cdiv(M, tc.bm);
   p.tiles_n = (int32_t)cdiv(N, tc.bn);
   p.splitk = best_split;
@@ -378,17 +360,13 @@ inline int plan_pair(const qb_tensor_t *A, const int32_t *la,
   plan.streamk = 0;
   plan.flags_clean = false;
   {
-    static const int sk_env = [] {
-      const char *e = getenv("QB_STREAMK");
-      return e ? atoi(e) : 1;
-    }();
     // one persistent CTA per SM: owners spin on their peers' flags, so every
     // CTA of the grid must be resident at once
     const int G = nsm;
     const int64_t tiles = (int64_t)p.tiles_m * p.tiles_n;
     const int64_t kblocks = cdiv(Kh, tc.bk);
     const double eff = (double)(tiles * p.splitk) / (double)(cdiv(tiles * p.splitk, G) * G);
-    if (sk_env && cfg == 0 && p.nbatch == 1 && tiles >= 32 && tiles * kblocks >= 8LL * G &&
+    if (cfg == 0 && p.nbatch == 1 && tiles >= 32 && tiles * kblocks >= 8LL * G &&
         (eff < 0.93 || p.splitk > 1)) {
       plan.streamk = G;
       p.splitk = 1;
@@ -396,11 +374,8 @@ inline int plan_pair(const qb_tensor_t *A, const int32_t *la,
       // fix-up (wait + collect the peers' partial tiles) + epilogue of a
       // shared tile cost its owner about head_us = this many k-blocks; it gets
       // that much less of the main loop.  9 us is an estimate that has not
-      // been measured on the H100 (QB_SK_HEAD_US overrides it for tuning)
-      static const int head_us = [] {
-        const char *e = getenv("QB_SK_HEAD_US");
-        return e ? atoi(e) : 9;
-      }();
+      // been measured on the H100
+      constexpr double head_us = 9.0;
       const double kb_us = (double)tc.bm * tc.bn * tc.bk / (0.9 * kDmmaFmaPerSmUs);
       int64_t H = (int64_t)(head_us / kb_us + 0.5);
       const int64_t share = tiles * (kblocks + H) / G;
@@ -419,13 +394,6 @@ inline int a_kmajor(const ContractParams &p) {
 }
 inline int b_kmajor(const ContractParams &p) {
   return (p.vecB == 2) || (p.vecB == 0 && p.thrB == 1);
-}
-inline bool layout_spec() {
-  static const bool on = [] {
-    const char *e = getenv("QB_LAYOUT_SPEC");
-    return e ? atoi(e) != 0 : true;
-  }();
-  return on;
 }
 
 // Which kernel a contraction runs.  select_route (api.cu) decides the engine;
@@ -447,7 +415,7 @@ struct Route {
   int streamk;    // stream-K grid (CTAs), 0 otherwise
   int sk_head;    // stream-K cost of a tile's fix-up, in k-blocks
   int bk;         // DMMA k-block depth
-  int layout;     // cfg 0, real: a_kmajor * 2 + b_kmajor; -1: runtime layout
+  int layout;     // cfg 0, real: a_kmajor * 2 + b_kmajor; -1 otherwise
   int launches;   // kernels launched (beta = 0)
   int stream_k;   // streaming engine: compiled (KMAX, NMAX) variant, 0 otherwise
   int stream_n;
@@ -456,7 +424,7 @@ struct Route {
 // DMMA part of a route.  A stream-K grid needs the workspace scratch that the
 // planner sized for it (internal GEMMs without scratch run classic launches).
 inline Route dmma_route(const PairPlan &plan, bool have_scratch) {
-  Route r{ROUTE_DMMA, plan.cfg, plan.p.splitk, 0, 0, tile_cfg(plan.cfg).bk, -1, 1};
+  Route r{ROUTE_DMMA, plan.cfg, plan.p.splitk, 0, 0, kTileCfgs[plan.cfg].bk, -1, 1};
   const bool cplx = dtype_is_complex(plan.dtype);
   if (plan.streamk > 0 && have_scratch) {
     r.kind = ROUTE_DMMA_STREAMK;
@@ -466,7 +434,7 @@ inline Route dmma_route(const PairPlan &plan, bool have_scratch) {
   } else if (r.splitk > 1) {
     r.launches = 2;  // + splitk_reduce_f64_kernel
   }
-  if (plan.cfg == 0 && !cplx && layout_spec())
+  if (plan.cfg == 0 && !cplx)
     r.layout = a_kmajor(plan.p) * 2 + b_kmajor(plan.p);
   return r;
 }

@@ -5,8 +5,7 @@
 // into the epilogue, so that a truncated split is ONE library call that
 // writes exactly the kept factors.
 //
-// Round structure (what changed against the round-1 kernel, which is kept in
-// linalg.cu as the `QB_JAC_MODE=v1` A/B reference):
+// Round structure:
 //
 //   * a sweep is cut into INDEPENDENT sub-tournaments (2 or 4 groups of column
 //     blocks: round robin inside every group, then bipartite rounds between
@@ -15,8 +14,8 @@
 //     (2-4 CTAs per SM), so the latency-bound 32 x 32 eigen-solve of one pair
 //     overlaps the DMMA-bound Gram / apply phases of others -- the phases of
 //     one launch all coincide, which is what left the tensor pipe 33 % busy;
-//   * a column-block pair is owned by a CLUSTER of 4 or 8 CTAs (rows dealt in
-//     chunks), 256 or 512 CTAs per round over all streams: every SM busy;
+//   * a column-block pair is owned by a CLUSTER of 2 CTAs (rows dealt in
+//     64-row chunks, 4 cp.async stages);
 //   * the partial Gram is computed with each warp owning one 16 x 8 output
 //     tile over all rows of the chunk: no cross-warp reduction, only the
 //     fixed-order cluster reduction through distributed shared memory;
@@ -27,7 +26,6 @@
 #include <cooperative_groups.h>
 #include <math.h>
 #include <stdlib.h>
-#include <time.h>
 
 #include <algorithm>
 #include <vector>
@@ -35,10 +33,6 @@
 #include "internal.h"
 
 namespace qb {
-
-int svd_tall_f64_v1(int64_t m, int64_t n, const double *X, double *U, double *S,
-                    double *VH, double *ws, int *sweeps_out, cudaStream_t st);
-int64_t svd_v1_workspace_doubles(int64_t m, int64_t n);
 
 namespace jac2 {
 
@@ -480,14 +474,6 @@ __global__ void __launch_bounds__(256, MINB) jacobi_round_kernel(const Params P)
   J2_TRACE(6);
 }
 
-// de-phases the independent streams of a sweep: stream g starts its rounds
-// g * stagger later, so that the L2-bound Gram / apply phases of one stream
-// fall into the eigen-solve phase of another instead of all coinciding
-__global__ void delay_kernel(unsigned long long ns) {
-  const unsigned long long t0 = now_ns();
-  while (now_ns() - t0 < ns) __nanosleep(200);
-}
-
 // ---------------------------------------------------------------- schedule ---
 // A sweep as a list of phases; inside a phase `ngroups` independent launch
 // sequences (one per stream), each a list of rounds, each round a list of
@@ -715,32 +701,20 @@ static bool geometry(int64_t m, int64_t n, Geom &g) {
   return true;
 }
 
-struct Config { int cs, ch, stg, groups; };
+// launch geometry of a round: CTAs per cluster, rows per streamed chunk and
+// cp.async stages (jacobi_round_kernel<kJacCh, kJacStg, 1>)
+constexpr int kJacCs = 2, kJacCh = 64, kJacStg = 4;
 
-static Config pick_config(int nblk) {
-  static const Config env = [] {
-    Config c{0, 0, 0, 0};
-    if (const char *e = getenv("QB_JAC_CS")) c.cs = atoi(e);
-    if (const char *e = getenv("QB_JAC_CH")) c.ch = atoi(e);
-    if (const char *e = getenv("QB_JAC_STG")) c.stg = atoi(e);
-    if (const char *e = getenv("QB_JAC_GROUPS")) c.groups = atoi(e);
-    return c;
-  }();
-  Config c{2, 64, 4, 4};
-  if (nblk < 64) c.groups = 2;
-  if (nblk < 16) c.groups = 1;
-  if (env.cs == 1 || env.cs == 2 || env.cs == 4 || env.cs == 8) c.cs = env.cs;
-  if (env.ch == 32 || env.ch == 64) c.ch = env.ch;
-  if (env.stg >= 2 && env.stg <= 4) c.stg = env.stg;
-  if (env.groups == 1 || env.groups == 2 || env.groups == 4) c.groups = env.groups;
-  while (c.groups > 1 && (nblk < 4 * c.groups || nblk % (2 * c.groups))) c.groups /= 2;
-  return c;
+// independent sub-tournaments (streams) of a sweep over nblk column blocks
+static int pick_groups(int nblk) {
+  int groups = nblk < 16 ? 1 : (nblk < 64 ? 2 : 4);
+  while (groups > 1 && (nblk < 4 * groups || nblk % (2 * groups))) groups /= 2;
+  return groups;
 }
 
-template <int CH, int STG, int MINB>
-static int launch_round(const Params &P, int npairs, int cs, cudaStream_t st) {
-  auto kern = jacobi_round_kernel<CH, STG, MINB>;
-  const size_t smem = sizeof(Smem<CH, STG>);
+static int launch_round(const Params &P, int npairs, cudaStream_t st) {
+  auto kern = jacobi_round_kernel<kJacCh, kJacStg, 1>;
+  const size_t smem = sizeof(Smem<kJacCh, kJacStg>);
   static bool attr_set = false;
   if (!attr_set) {
     QB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -748,13 +722,13 @@ static int launch_round(const Params &P, int npairs, int cs, cudaStream_t st) {
     attr_set = true;
   }
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(npairs * cs), 1, 1);
+  cfg.gridDim = dim3((unsigned)(npairs * kJacCs), 1, 1);
   cfg.blockDim = dim3(256, 1, 1);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)cs;
+  attr[0].val.clusterDim.x = (unsigned)kJacCs;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
@@ -762,17 +736,6 @@ static int launch_round(const Params &P, int npairs, int cs, cudaStream_t st) {
   QB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, P));
   g_launch_count.fetch_add(1, std::memory_order_relaxed);
   return 0;
-}
-
-static int launch_round_cfg(const Config &c, const Params &P, int npairs, cudaStream_t st) {
-  if (c.ch == 64) {
-    if (c.stg >= 4) return launch_round<64, 4, 1>(P, npairs, c.cs, st);
-    if (c.stg == 3) return launch_round<64, 3, 2>(P, npairs, c.cs, st);
-    return launch_round<64, 2, 2>(P, npairs, c.cs, st);
-  }
-  if (c.stg >= 4) return launch_round<32, 4, 3>(P, npairs, c.cs, st);
-  if (c.stg == 3) return launch_round<32, 3, 3>(P, npairs, c.cs, st);
-  return launch_round<32, 2, 4>(P, npairs, c.cs, st);
 }
 
 struct SideStreams {
@@ -797,7 +760,7 @@ static SideStreams &side_streams() {
 
 // Sweeps 1 .. kGraphSweeps - 1 of a multi-group schedule replay a cached CUDA
 // graph (QB_JAC_GRAPH=0: direct launches); later sweeps run direct launches
-// with fuller inner solves (inner_max >= 4).
+// with fuller inner solves (inner_max = 4).
 constexpr int kGraphSweeps = 25;
 static bool sweep_graph_eligible(int ngroups) {
   static const bool use_graph = [] {
@@ -812,9 +775,8 @@ static bool sweep_graph_eligible(int ngroups) {
 static int jacobi_iterate(double *W, double *Z, int64_t n, int64_t npad, int2 *d_pairs,
                           int *flag, const double *negl, int *sweeps_out, cudaStream_t st) {
   const int nblk = (int)(npad / JB);
-  const Config cfg = pick_config(nblk);
   Schedule sched;
-  build_schedule(nblk, cfg.groups, sched);
+  build_schedule(nblk, pick_groups(nblk), sched);
   QB_CUDA_CHECK(cudaMemcpyAsync(d_pairs, sched.pairs.data(), sizeof(int2) * sched.pairs.size(),
                                 cudaMemcpyHostToDevice, st));
   Params P;
@@ -824,21 +786,12 @@ static int jacobi_iterate(double *W, double *Z, int64_t n, int64_t npad, int2 *d
   P.flag = flag;
   P.offmax = reinterpret_cast<unsigned long long *>(flag + 2);
   P.trace = trace_buffer() ? trace_buffer() + 16 * 8192 : nullptr;
-  static const int inner0 = [] { const char *e = getenv("QB_JAC_INNER"); return e ? atoi(e) : 1; }();
-  static const long stagger_ns = [] { const char *e = getenv("QB_JAC_STAGGER"); return e ? atol(e) : 0L; }();
   SideStreams &SS = side_streams();
   const bool multi = sched.ngroups > 1;
   int sweeps = 0;
   const int max_sweeps = 60;
   int slot = 0;
   bool done = false;
-  static const bool prof = getenv("QB_JAC_PROFILE") != nullptr;
-  double t_issue = 0.0, t_wait = 0.0;
-  auto wall = [] {
-    timespec ts;
-    clock_gettime(CLOCK_MONOTONIC, &ts);
-    return ts.tv_sec + 1e-9 * ts.tv_nsec;
-  };
   // one sweep = every phase forked over the group streams and joined again;
   // `origin` is the stream the forks hang off (the caller's, or the capture
   // stream when the sweep is recorded into a CUDA graph)
@@ -848,14 +801,10 @@ static int jacobi_iterate(double *W, double *Z, int64_t n, int64_t npad, int2 *d
       for (size_t g = 0; g < ph.rounds.size(); ++g) {
         cudaStream_t gs = multi ? SS.s[g % 4] : origin;
         if (multi) QB_CUDA_CHECK(cudaStreamWaitEvent(gs, SS.fork, 0));
-        if (multi && g > 0 && stagger_ns > 0) {
-          delay_kernel<<<1, 1, 0, gs>>>((unsigned long long)g * stagger_ns);
-          QB_LAUNCH_CHECK();
-        }
         for (const auto &rd : ph.rounds[g]) {
           P.pairs = d_pairs + rd.first;
           P.trace_slot = (slot++) & 1023;
-          int rc = launch_round_cfg(cfg, P, rd.second, gs);
+          int rc = launch_round(P, rd.second, gs);
           if (rc) return rc;
         }
         if (multi) {
@@ -869,27 +818,23 @@ static int jacobi_iterate(double *W, double *Z, int64_t n, int64_t npad, int2 *d
   // Sweeps after the first replay a CUDA graph of the sweep (the launch
   // sequence of a sweep is fixed: ~500 cluster launches on 4 streams cost more
   // host time than the device needs to run them).  The executable graph is
-  // cached per (buffers, size, configuration): a DMRG sweep factors the same
-  // shape in the same workspace at every site.
+  // cached per (buffers, size; the schedule is a function of npad): a DMRG
+  // sweep factors the same shape in the same workspace at every site.
   struct SweepGraph {
     cudaGraphExec_t exec = nullptr;
     const void *W = nullptr, *Z = nullptr, *pairs = nullptr;
     int64_t n = 0, npad = 0;
-    Config cfg{0, 0, 0, 0};
-    int inner = 0;
-    long stagger = 0;
   };
   static thread_local SweepGraph SG;
   const bool graph_ok = sweep_graph_eligible(sched.ngroups);
   auto graph_matches = [&]() {
     return SG.exec && SG.W == W && SG.Z == Z && SG.pairs == d_pairs && SG.n == n &&
-           SG.npad == npad && SG.cfg.cs == cfg.cs && SG.cfg.ch == cfg.ch &&
-           SG.cfg.stg == cfg.stg && SG.cfg.groups == cfg.groups && SG.inner == inner0 &&
-           SG.stagger == stagger_ns;
+           SG.npad == npad;
   };
   for (; sweeps < max_sweeps && !done; ++sweeps) {
-    const double t0 = wall();
-    P.inner_max = (sweeps < kGraphSweeps) ? inner0 : std::max(inner0, 4);
+    // one inner sweep per visit is fastest; fall back to fuller inner solves
+    // if the outer iteration is unusually slow
+    P.inner_max = (sweeps < kGraphSweeps) ? 1 : 4;
     QB_CUDA_CHECK(cudaMemsetAsync(flag, 0, 16, st));
     bool launched = false;
     if (graph_ok && sweeps >= 1 && sweeps < kGraphSweeps) {
@@ -904,8 +849,7 @@ static int jacobi_iterate(double *W, double *Z, int64_t n, int64_t npad, int2 *d
         if (ok) ok = cudaGraphInstantiate(&SG.exec, gr, 0) == cudaSuccess;
         if (gr) cudaGraphDestroy(gr);
         if (ok) {
-          SG.W = W; SG.Z = Z; SG.pairs = d_pairs; SG.n = n; SG.npad = npad; SG.cfg = cfg;
-          SG.inner = inner0; SG.stagger = stagger_ns;
+          SG.W = W; SG.Z = Z; SG.pairs = d_pairs; SG.n = n; SG.npad = npad;
         } else {
           cudaGetLastError();     // clear; fall back to direct launches
           SG.exec = nullptr;
@@ -923,9 +867,7 @@ static int jacobi_iterate(double *W, double *Z, int64_t n, int64_t npad, int2 *d
     }
     struct { int flag; int pad; unsigned long long off; } h = {0, 0, 0};
     QB_CUDA_CHECK(cudaMemcpyAsync(&h, flag, 16, cudaMemcpyDeviceToHost, st));
-    const double t1 = wall();
     QB_CUDA_CHECK(cudaStreamSynchronize(st));
-    t_issue += t1 - t0; t_wait += wall() - t1;
     // converged when a whole sweep rotated nothing.  (Stopping one sweep
     // earlier because the largest scaled off-diagonal was tiny is NOT safe:
     // for close singular values the rotation ANGLES stay large however small
@@ -933,10 +875,6 @@ static int jacobi_iterate(double *W, double *Z, int64_t n, int64_t npad, int2 *d
     // measured: 1e-11 .. 2e-10 loss of orthogonality on degenerate spectra.)
     if (!h.flag) done = true;
   }
-  if (prof)
-    fprintf(stderr, "[qb jacobi] n=%lld sweeps=%d groups=%d cs=%d: host issue %.1f ms, "
-            "waiting for the device %.1f ms\n", (long long)n, sweeps, sched.ngroups, cfg.cs,
-            t_issue * 1e3, t_wait * 1e3);
   if (sweeps_out) *sweeps_out = sweeps;
   if (!done) {
     set_error("qb_svd: Jacobi did not converge in %d sweeps", max_sweeps);
@@ -1178,8 +1116,7 @@ int64_t qb_svd_workspace(int dtype, int64_t m, int64_t n) {
   jac2::Geom g;
   const int64_t mm = std::max(m, n), nn = std::min(m, n);
   if (!jac2::geometry(mm, nn, g)) return -2;
-  const int64_t v1 = svd_v1_workspace_doubles(mm, nn);
-  return std::max(g.total, v1) * 8;
+  return g.total * 8;
 }
 
 static int svd_check(const char *who, int dtype, int64_t m, int64_t n, void *workspace,
@@ -1210,18 +1147,10 @@ int qb_svd(int dtype, int64_t m, int64_t n, const void *X, void *U, void *S,
   if (m <= 0 || n <= 0) return 0;
   int rc = svd_check("qb_svd", dtype, m, n, workspace, workspace_bytes);
   if (rc) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  double *ws = static_cast<double *>(workspace);
-  static const bool v1 = [] {
-    const char *e = getenv("QB_JAC_MODE");
-    return e && !strcmp(e, "v1");
-  }();
-  if (v1)
-    return svd_tall_f64_v1(m, n, (const double *)X, (double *)U, (double *)S,
-                           (double *)VH, ws, sweeps_out, st);
   return svd_trunc_tall(m, n, (const double *)X, -1.0, 0, -1, QB_ABSORB_FULL, 0,
                         (double *)U, (double *)S, (double *)VH, nullptr, nullptr, nullptr,
-                        ws, sweeps_out, st);
+                        static_cast<double *>(workspace), sweeps_out,
+                        static_cast<cudaStream_t>(stream));
 }
 
 // TEST / debug entry, host only: the sweep schedule of the Jacobi SVD for
@@ -1264,14 +1193,13 @@ int qb_svd_route(int64_t m, int64_t n, int absorb, int64_t *out) {
     return -8;
   }
   const int nblk = (int)(g.npad / jac2::JB);
-  const jac2::Config c = jac2::pick_config(nblk);
   jac2::Schedule S;
-  jac2::build_schedule(nblk, c.groups, S);
+  jac2::build_schedule(nblk, jac2::pick_groups(nblk), S);
   int64_t rounds = 0;
   for (const auto &ph : S.phases)
     for (const auto &gr : ph.rounds) rounds += (int64_t)gr.size();
-  out[0] = g.npad; out[1] = nblk; out[2] = S.ngroups; out[3] = c.cs; out[4] = c.ch;
-  out[5] = c.stg; out[6] = epilogue_kind(absorb);
+  out[0] = g.npad; out[1] = nblk; out[2] = S.ngroups; out[3] = jac2::kJacCs;
+  out[4] = jac2::kJacCh; out[5] = jac2::kJacStg; out[6] = epilogue_kind(absorb);
   out[7] = jac2::sweep_graph_eligible(S.ngroups) ? jac2::kGraphSweeps - 1 : 0;
   out[8] = q.panel_mask; out[9] = q.wy_t; out[10] = rounds;
   return 0;

@@ -35,13 +35,14 @@ def _resource_usage():
 
 
 @pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="cuobjdump not found")
-def test_large_dmma_tiles_do_not_spill():
+def test_large_dmma_tiles_bk32_only_and_do_not_spill():
     # mangled contract_f64_kernel / contract_f64_streamk_kernel<128, 128, ...>
     pat = re.compile(r"_ZN2qb(19contract_f64_kernel|27contract_f64_streamk_kernel)"
                      r"ILi128ELi128E")
     large = {n: u for n, u in _resource_usage().items() if pat.match(n)}
-    # 2 BK depths x (4 layouts + runtime layout + complex) x 2 launch modes
-    assert len(large) == 24, sorted(large)
+    # 4 layouts + complex, BK 32, x 2 launch modes
+    assert len(large) == 10, sorted(large)
+    assert all(re.search(r"ILi128ELi128ELi32ELi2ELi4ELi3E", n) for n in large), sorted(large)
     assert all(reg <= 255 for reg, _ in large.values())
     # the stream-K kernels also carry the segment loop's state across the tile;
     # up to 96 B of it lives on the stack, reloaded around the epilogue and

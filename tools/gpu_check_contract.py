@@ -175,17 +175,6 @@ def main():
     bc = torch.randn(n, n, dtype=torch.complex128, device=dev)
     tmin, _ = timeit(lambda: contract_pair(ac, [0, 1], bc, [1, 2], [0, 2]))
     print(f"zgemm 2048^3: {tmin:.3f} ms {8 * n**3 / tmin / 1e9:.2f} TFLOP/s(real)", flush=True)
-    # tile config sweep on NN gemm (separate processes: the override is read once)
-    if "QB_FORCE_CFG" not in os.environ:
-        import subprocess
-        for cfg in (0, 1):
-            env = dict(os.environ, QB_FORCE_CFG=str(cfg))
-            code = ("import torch,sys;sys.path.insert(0,'.');from quimb_b200.contract import contract_pair;"
-                    "n=4096;a=torch.randn(n,n,dtype=torch.float64,device='cuda');b=torch.randn(n,n,dtype=torch.float64,device='cuda');"
-                    "c=torch.empty_like(a);f=lambda:contract_pair(a,[0,1],b,[1,2],[0,2],out=c);f();torch.cuda.synchronize();"
-                    "e0=torch.cuda.Event(enable_timing=True);e1=torch.cuda.Event(enable_timing=True);e0.record();f();f();f();e1.record();torch.cuda.synchronize();"
-                    "t=e0.elapsed_time(e1)/3;print('cfg',%d,t,'ms',2*n**3/t/1e9,'TFLOP/s')" % cfg)
-            subprocess.run([sys.executable, "-c", code], env=env)
     os.makedirs("gpurun_out", exist_ok=True)
     json.dump(res, open("gpurun_out/check_contract.json", "w"))
     return 0 if ok else 1

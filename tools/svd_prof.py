@@ -4,9 +4,6 @@ from its in-kernel %globaltimer stamps (cluster 0 of every launch).
 
 phases: 0 entry, 1 Gram streamed, 2 Gram reduced over the cluster + off-norm,
         3 32x32 eigen-solve done, 4 sorted, 5 rotation applied, 6 cluster exit
-Kernel configuration through the environment (read once per process):
-QB_JAC_MODE=v1 (round-1 kernel) | QB_JAC_CS (cluster size) QB_JAC_CH (rows per
-chunk) QB_JAC_STG (stages) QB_JAC_GROUPS (independent streams).
 """
 import ctypes
 import json
@@ -33,10 +30,7 @@ for _ in range(3):
     U, s, VH, sw = qb.linalg.svd(X, return_sweeps=True)
     e1.record(); torch.cuda.synchronize()
     ts.append(e0.elapsed_time(e1))
-out = {"n": n, "sweeps": sw, "ms": min(ts), "ms_all": ts,
-       "cfg": {k: os.environ.get(k) for k in ("QB_JAC_MODE", "QB_JAC_CS", "QB_JAC_CH",
-                                               "QB_JAC_STG", "QB_JAC_GROUPS", "QB_JAC_INNER")
-               if os.environ.get(k)}}
+out = {"n": n, "sweeps": sw, "ms": min(ts), "ms_all": ts}
 # fused truncated split (DMRG shape: keep half, absorb right)
 for name, code in (("trunc_ms", 1), ("trunc_left_ms", -1), ("trunc_both_ms", 0)):
     ts2 = []

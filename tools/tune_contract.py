@@ -1,30 +1,25 @@
-"""Tuning probe for the DMMA contraction kernel (GPU box only).
+"""Time the DMMA contraction kernel on plain fp64 GEMMs (GPU only): 4096³ and
+two shapes of the chi=1024 MPS-norm step.  Prints one JSON line per shape
+(ms per call, TFLOP/s, and for the smaller shapes the max error against
+torch.matmul).
 
-Each variant is selected by environment variables that the library reads once
-per process, so every variant runs in its own subprocess.  The DBG variants
-compute garbage; only their timing is meaningful (which part of the main loop
-costs what).
-
-  python tools/tune_contract.py            # drive all variants
-  python tools/tune_contract.py --one      # (internal) time the current env
+  python tools/tune_contract.py [--out result.json]
 """
 import json
 import os
-import subprocess
 import sys
-import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
+SHAPES = [[4096, 4096, 4096], [1024, 2048, 1024], [1024, 1024, 2048]]  # (M, N, K)
 
-def one():
+
+def main():
     import torch
-    import quimb_b200 as qb
     from quimb_b200.contract import contract_pair
     dev = torch.device("cuda:0")
     out = {}
-    shapes = json.loads(os.environ.get("TUNE_SHAPES", "[[4096,4096,4096]]"))
-    for (M, N, K) in shapes:
+    for (M, N, K) in SHAPES:
         g = torch.Generator(device=dev); g.manual_seed(1)
         A = torch.randn((M, K), dtype=torch.float64, device=dev, generator=g)
         B = torch.randn((K, N), dtype=torch.float64, device=dev, generator=g)
@@ -39,42 +34,13 @@ def one():
             contract_pair(A, [0, 1], B, [1, 2], [0, 2], out=C)
         e1.record(); torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / reps
-        err = None
-        if os.environ.get("QB_DBG", "0") == "0" and M <= 2048:
-            err = float((C - A @ B).abs().max().item())
-        out[f"{M}x{N}x{K}"] = {"ms": round(ms, 4), "tflops": round(2.0 * M * N * K / ms / 1e9, 2),
-                               "err": err}
-    print("TUNE " + json.dumps(out))
-
-
-VARIANTS = [
-    ("bk16 classic", {"QB_STREAMK": "0", "QB_CFG0_BK": "16"}),
-    ("bk32 classic", {"QB_STREAMK": "0", "QB_CFG0_BK": "32"}),
-    ("bk16 streamk", {"QB_CFG0_BK": "16"}),
-    ("bk32 streamk", {"QB_CFG0_BK": "32"}),
-    ("bk32 streamk runtime layouts", {"QB_CFG0_BK": "32", "QB_LAYOUT_SPEC": "0"}),
-]
-
-
-def main():
-    if "--one" in sys.argv:
-        return one()
-    shapes = [[4096, 4096, 4096], [1024, 2048, 1024], [1024, 1024, 2048]]
-    res = {}
-    for name, env in VARIANTS:
-        e = dict(os.environ); e.update(env); e["TUNE_SHAPES"] = json.dumps(shapes)
-        t0 = time.time()
-        try:
-            pr = subprocess.run([sys.executable, os.path.abspath(__file__), "--one"], env=e,
-                                capture_output=True, text=True, timeout=120)
-            line = [l for l in pr.stdout.splitlines() if l.startswith("TUNE ")]
-            res[name] = json.loads(line[0][5:]) if line else {"error": pr.stderr[-400:]}
-        except subprocess.TimeoutExpired:
-            res[name] = {"error": "timeout"}
-        print(f"{name:34s} {json.dumps(res[name])}  ({time.time() - t0:.0f}s)", flush=True)
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/tune_contract.json", "w") as fh:
-        json.dump(res, fh, indent=1)
+        err = float((C - A @ B).abs().max().item()) if M <= 2048 else None
+        out[f"{M}x{N}x{K}"] = r = {"ms": round(ms, 4),
+                                   "tflops": round(2.0 * M * N * K / ms / 1e9, 2), "err": err}
+        print(json.dumps({f"{M}x{N}x{K}": r}), flush=True)
+    if "--out" in sys.argv:
+        with open(sys.argv[sys.argv.index("--out") + 1], "w") as fh:
+            json.dump(out, fh, indent=1)
 
 
 if __name__ == "__main__":
