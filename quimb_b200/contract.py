@@ -28,6 +28,39 @@ def _workspace(nbytes, device):
     return buf
 
 
+def _scratch_dicts():
+    """Every per-(device, stream) scratch cache of the package; keys end with
+    the stream handle."""
+    from . import lanczos, linalg, ops
+    return (_WS, linalg._WS, ops._DOT_WS, lanczos._MD_WS)
+
+
+def capture_graph(fn):
+    """Capture ``fn()`` into a CUDA graph that owns its scratch; returns
+    ``(graph, value of the captured call, scratch buffers)``.
+
+    ``fn`` first runs eagerly on a new side stream and is then captured on
+    that same stream, so every scratch buffer the captured launches use is
+    allocated (and its zero fill has run) before capture begins.  Those
+    buffers are then taken out of the per-stream caches: the caller keeps
+    them alive with the graph, and no later eager call or capture -- torch
+    recycles stream handles -- can reach them."""
+    dev = torch.device("cuda", torch.cuda.current_device())
+    st = torch.cuda.Stream(device=dev)
+    st.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(st):
+        fn()                              # warm-up: scratch, kernel attributes
+    torch.cuda.synchronize()
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph, stream=st):
+        out = fn()
+    scratch = []
+    for d in _scratch_dicts():
+        for key in [k for k in d if k[-1] == st.cuda_stream]:
+            scratch.append(d.pop(key))
+    return graph, out, scratch
+
+
 _WIDE = {torch.float32: torch.float64, torch.complex64: torch.complex128}
 
 

@@ -48,11 +48,13 @@ _NCV_MAX = 64
 
 
 def _md_ws(dev):
-    ws = _MD_WS.get(dev.index)
+    """Partials of ``qb_multi_dot``, one buffer per (device, stream)."""
+    key = (dev.index, torch.cuda.current_stream(dev).cuda_stream)
+    ws = _MD_WS.get(key)
     if ws is None:
         ws = torch.empty(_lib.load().qb_multi_dot_workspace(), dtype=torch.uint8,
                          device=dev)
-        _MD_WS[dev.index] = ws
+        _MD_WS[key] = ws
     return ws
 
 

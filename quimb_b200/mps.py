@@ -93,7 +93,9 @@ def stream_sites(sites, copy_stream=None, depth=3):
     allocator traffic on the path, and a buffer is overwritten only after the
     main stream has passed the work that consumed it (event recorded when the
     consumer asks for the next site).  The yielded device tensors are therefore
-    TRANSIENT views: valid until ``depth`` further sites have been requested."""
+    TRANSIENT views: valid until ``depth`` further sites have been requested.
+    A consumer that stops early closes the generator: that orders the main
+    stream after the copies still in flight into the ring."""
     import torch
     if not any(_is_host(s) for s in sites):
         yield from sites
@@ -142,25 +144,31 @@ def stream_sites(sites, copy_stream=None, depth=3):
 
     n = len(sites)
     nxt = 0
-    while nxt < n and len(pending) < depth:
-        pending.append(issue(nxt))
-        nxt += 1
-    prev = None
-    while pending:
-        d, ev, where = pending.pop(0)
-        if prev is not None:
-            # everything the consumer enqueued for the previous site is on the
-            # main stream by now: its staging slot may be refilled after that
-            e = torch.cuda.Event()
-            e.record(main)
-            consumed[prev[0]][prev[1]] = e
-        if nxt < n:
+    try:
+        while nxt < n and len(pending) < depth:
             pending.append(issue(nxt))
             nxt += 1
-        if ev is not None:
-            main.wait_event(ev)
-        prev = where
-        yield d
+        prev = None
+        while pending:
+            d, ev, where = pending.pop(0)
+            if prev is not None:
+                # everything the consumer enqueued for the previous site is on
+                # the main stream by now: its staging slot may be refilled after
+                main_done = torch.cuda.Event()
+                main_done.record(main)
+                consumed[prev[0]][prev[1]] = main_done
+            if nxt < n:
+                pending.append(issue(nxt))
+                nxt += 1
+            if ev is not None:
+                main.wait_event(ev)
+            prev = where
+            yield d
+    finally:
+        # a consumer that stops early leaves copies into the shared ring in
+        # flight: order the main stream after them, so the next call (whose
+        # side stream starts behind the main stream) cannot race them
+        main.wait_stream(side)
 
 
 def mps_norm2(sites, shape="lrp", copy_stream=None):
@@ -169,13 +177,17 @@ def mps_norm2(sites, shape="lrp", copy_stream=None):
     returns a 0-d device Array."""
     n = len(sites)
     E = None
-    for i, s in enumerate(stream_sites(sites, copy_stream)):
-        A = site_lpr(s, shape, i, n)
-        if E is None:
-            E = ops.ones((A.shape[0], A.shape[0]), dtype=A.dtype, device=A.device)
-            if A.shape[0] != 1:
-                E = ops.eye(A.shape[0], dtype=A.dtype, device=A.device)
-        E = norm_step(E, A)
+    staged = stream_sites(sites, copy_stream)
+    try:
+        for i, s in enumerate(staged):
+            A = site_lpr(s, shape, i, n)
+            if E is None:
+                E = ops.ones((A.shape[0], A.shape[0]), dtype=A.dtype, device=A.device)
+                if A.shape[0] != 1:
+                    E = ops.eye(A.shape[0], dtype=A.dtype, device=A.device)
+            E = norm_step(E, A)
+    finally:
+        staged.close()           # an error midway: settle the staging copies now
     if E.shape != (1, 1):
         return ops.trace(E)
     return E.reshape(())
@@ -380,10 +392,12 @@ class ChainPlan:
     and ``__call__`` replays the whole chain -- hundreds of launches of the
     contraction kernel, their workspaces and intermediates -- with one graph
     launch and no host work per site.  Outputs are the plan's own buffers
-    (clone to keep across replays)."""
+    (clone to keep across replays); so is the contraction scratch the graph
+    uses (``contract.capture_graph``), so plans may be replayed in any order
+    and on different streams at once."""
 
     def __init__(self, sites, mpo=None, shape="lrp", mpo_shape="lrud", kind="norm"):
-        import torch
+        from .contract import capture_graph
         if kind not in ("norm", "expec", "left_envs", "right_envs"):
             raise ValueError(f"unknown plan kind {kind!r}")
         if kind == "expec" and mpo is None:
@@ -392,11 +406,7 @@ class ChainPlan:
         self.sites = [ops.materialize(ops.asarray(s), force=True) for s in sites]
         self.mpo = None if mpo is None else [ops.materialize(ops.asarray(w), force=True)
                                              for w in mpo]
-        self._run()                       # warm-up: workspaces, kernel attributes
-        torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.out = self._run()
+        self.graph, self.out, self._scratch = capture_graph(self._run)
         self.replays = 0
 
     def _run(self):

@@ -500,11 +500,14 @@ _DOT_WS = {}
 
 
 def _dot_ws(dev):
-    ws = _DOT_WS.get(dev.index)
+    """Stage-1 partials of ``qb_dot``, one buffer per (device, stream): dot
+    products running on two streams at once must not share them."""
+    key = (dev.index, torch.cuda.current_stream(dev).cuda_stream)
+    ws = _DOT_WS.get(key)
     if ws is None:
         n = _lib.load().qb_dot_workspace(0)
         ws = torch.empty(n, dtype=torch.uint8, device=dev)
-        _DOT_WS[dev.index] = ws
+        _DOT_WS[key] = ws
     return ws
 
 

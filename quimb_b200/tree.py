@@ -667,22 +667,21 @@ class GraphedContraction:
     (tests/test_tensor/test_contract.py:155-175); here the cached object is
     the captured launch sequence itself, so a repeat contraction with new
     input values costs one graph launch.  Input arrays are copied into static
-    device buffers; the output buffer is reused (clone it to keep it).
+    device buffers; the output buffer is reused (clone it to keep it).  The
+    graph owns its scratch (``contract.capture_graph``), so plans may be
+    replayed in any order and on different streams at once.
     """
 
     def __init__(self, inputs, output, example_arrays, optimize="auto"):
-        import torch
+        from .contract import capture_graph
         arrays = [ops.materialize(ops.asarray(a), force=True) for a in example_arrays]
         self.inputs = [tuple(t) for t in inputs]
         self.output = tuple(output)
         self.tree = find_tree(self.inputs, self.output, _sizes(self.inputs, arrays),
                               optimize)
         self.static_in = arrays
-        execute(self.tree, self.static_in)          # warm-up: attributes, workspaces
-        torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.out = execute(self.tree, self.static_in)
+        self.graph, self.out, self._scratch = capture_graph(
+            lambda: execute(self.tree, self.static_in))
         self.n_nodes = len(self.tree.steps)
 
     def __call__(self, *arrays):
