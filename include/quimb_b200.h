@@ -184,6 +184,17 @@ int qb_contract_pair_route(const qb_tensor_t *A, const int32_t *labelsA,
                            int engine, int64_t *out16);
 
 /*
+ * Host-only: how the route of qb_contract_pair_route (engine = auto) feeds
+ * each operand into the DMMA large real tile.  out[0] / out[1] = feed of A /
+ * B: 1 affine (a per-thread address advanced by constant steps), 0 offset
+ * tables, -1 the route does not run the large real tile.
+ */
+int qb_contract_pair_feed(const qb_tensor_t *A, const int32_t *labelsA,
+                          const qb_tensor_t *B, const int32_t *labelsB,
+                          const qb_tensor_t *C, const int32_t *labelsC,
+                          int64_t *out2);
+
+/*
  * TEST / debug entry, host pointers only: runs the streaming engine's row
  * code (shared __host__ __device__ functions of contract_stream.cu) in a
  * host loop so that its index bookkeeping can be checked without a device.

@@ -340,6 +340,28 @@ def route_pair(a_shape, a_strides, la, b_shape, b_strides, lb, c_shape,
     return r
 
 
+FEEDS = {1: "affine", 0: "table", -1: None}
+
+
+def feed_pair(a_shape, a_strides, la, b_shape, b_strides, lb, c_shape,
+              c_strides, lc, dtype_code=_lib.QB_F64, ptrs=None):
+    """Host-only: how ``contract_pair`` (engine auto) gathers each operand
+    into the large real DMMA tile: ``"affine"`` (each thread's copies follow
+    constant strides, no offset tables), ``"table"`` (per-tile offset tables)
+    or None when the route does not run that tile.  ``ptrs`` as for
+    ``route_pair``."""
+    lib = _lib.load()
+    pa, pb, pc = ptrs if ptrs is not None else (0x10000000,) * 3
+    da = _lib.np_desc(a_shape, a_strides, dtype_code, pa)
+    db = _lib.np_desc(b_shape, b_strides, dtype_code, pb)
+    dc = _lib.np_desc(c_shape, c_strides, dtype_code, pc)
+    out = (ctypes.c_int64 * 2)()
+    rc = lib.qb_contract_pair_feed(da, _lib.labels(la), db, _lib.labels(lb),
+                                   dc, _lib.labels(lc), out)
+    _lib.check(rc, "qb_contract_pair_feed")
+    return {"A": FEEDS[out[0]], "B": FEEDS[out[1]]}
+
+
 def contract_batched(a_list, la, b_list, lb, lc, conj_a=False, conj_b=False):
     """Many independent contractions of identical signature in ONE launch
     (the small same-shape intermediates of MPS / PEPS / circuit sweeps).

@@ -183,6 +183,20 @@ int qb_contract_pair_route(const qb_tensor_t *A, const int32_t *la,
   return 0;
 }
 
+int qb_contract_pair_feed(const qb_tensor_t *A, const int32_t *la,
+                          const qb_tensor_t *B, const int32_t *lb,
+                          const qb_tensor_t *C, const int32_t *lc, int64_t *out) {
+  PairPlan plan;
+  int rc = plan_pair(A, la, B, lb, C, lc, 0, 0, plan);
+  if (rc) return rc;
+  const Route r = select_route(plan, QB_ENGINE_AUTO);
+  const bool large_real = (r.kind == ROUTE_DMMA || r.kind == ROUTE_DMMA_STREAMK) &&
+                          r.cfg == 0 && r.layout >= 0;
+  out[0] = large_real ? plan.p.feedA : -1;
+  out[1] = large_real ? plan.p.feedB : -1;
+  return 0;
+}
+
 int64_t qb_contract_pair_workspace(const qb_tensor_t *A, const int32_t *la,
                                    const qb_tensor_t *B, const int32_t *lb,
                                    const qb_tensor_t *C, const int32_t *lc,

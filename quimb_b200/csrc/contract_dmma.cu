@@ -9,6 +9,10 @@
 // gather straight from the strided tensors, so the index permutation that
 // numpy.tensordot performs as a separate transpose-copy
 // (quimb -> cotengra -> autoray do("tensordot")) is folded into the load.
+// Where the planner proves an operand's tile rows and k-blocks affine
+// (plan.h, affine_feed), the large real tile gathers it from one per-thread
+// address advanced by constant steps instead, and spends the registers the
+// tables held on prefetching the next k-step's fragments.
 //
 // Pipeline: STAGES-deep cp.async ring (16-byte copies whenever the planner
 // proved pairs of elements contiguous, 8-byte otherwise), one __syncthreads
@@ -135,6 +139,58 @@ __device__ __forceinline__ void load_tile_cplx(
   }
 }
 
+// Affine gather of one real operand tile (plan.h, affine_feed): copy i of
+// this thread reads src + i * step and lands at sm + i * sm_step bytes into
+// the stage; the next k-block starts kstep further on.  The addresses are
+// those the offset tables give, without the tables or predicates.
+struct AffineFeed {
+  const double *src;
+  int64_t step, kstep;
+  uint32_t sm, sm_step;
+  bool wide;  // 16-byte copies (vec != 0)
+};
+
+template <int ROWS, int BK, int NT, bool KMAJOR>
+__device__ __forceinline__ AffineFeed affine_setup(const double *base, int64_t rstep,
+                                                   int64_t kstep, int vec, int thr,
+                                                   int tid) {
+  // units: pairs of rows (vec 1) or of k (vec 2), single elements otherwise.
+  // NT is a multiple of both tile extents in units, so a thread keeps its
+  // inner coordinate and advances its outer one by NT / inner per copy
+  static_assert(NT % ROWS == 0 && NT % BK == 0 && (ROWS * BK / 2) % NT == 0,
+                "affine feed needs an affine thread walk");
+  const int ur = vec == 1 ? 2 : 1, uk = vec == 2 ? 2 : 1;
+  const int inner = thr ? BK / uk : ROWS / ur;
+  const int a = tid % inner, b = tid / inner, db = NT / inner;
+  const int ru = thr ? b : a, ku = thr ? a : b;
+  constexpr int s_row = KMAJOR ? BK + 4 : 1, s_k = KMAJOR ? 1 : ROWS + 4;
+  AffineFeed f;
+  f.src = base + ru * rstep + ku * kstep;
+  f.sm = (uint32_t)(ru * ur * s_row + ku * uk * s_k) * 8;
+  f.step = thr ? db * rstep : db * kstep;
+  f.sm_step = (uint32_t)(thr ? db * ur * s_row : db * uk * s_k) * 8;
+  f.kstep = (BK / uk) * kstep;
+  f.wide = vec != 0;
+  return f;
+}
+
+template <int ROWS, int BK, int NT>
+__device__ __forceinline__ void load_affine(uint32_t stage, const AffineFeed &f, int kb) {
+  // a running address, not unrolled: unrolled, ptxas keeps every copy's
+  // offset live across the k-loop (they do not depend on kb) and spills
+  const double *src = f.src + kb * f.kstep;
+  uint32_t dst = stage + f.sm;
+  if (f.wide) {
+#pragma unroll 1
+    for (int i = 0; i < ROWS * BK / 2 / NT; ++i, src += f.step, dst += f.sm_step)
+      cp_async16(dst, src, 16);
+  } else {
+#pragma unroll 1
+    for (int i = 0; i < ROWS * BK / NT; ++i, src += f.step, dst += f.sm_step)
+      cp_async8(dst, src, 8);
+  }
+}
+
 __device__ __forceinline__ double flip_sign(double v, unsigned mask_hi) {
   // mask_hi is 0 or 0x80000000
   return __hiloint2double(__double2hiint(v) ^ (int)mask_hi, __double2loint(v));
@@ -162,13 +218,17 @@ struct SkSeg {
   int seg;         // ordinal of this segment within the CTA (trace only)
 };
 
+// FEED: bit 0 / bit 1 = A / B gathered by the affine feed (real operands with
+// a compile-time layout only); 0 = offset tables for both
 template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
-          bool CPLX, int LA = -1, int LB = -1>
+          bool CPLX, int LA = -1, int LB = -1, int FEED = 0>
 __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
                                               int64_t zb, int ks, int64_t kbeg,
                                               int64_t kend, const SkSeg sk) {
   using Cfg = KernelCfg<BM, BN, BK, WARPS_M, WARPS_N, STAGES>;
   constexpr int NT = Cfg::NT;
+  constexpr bool AFA = (FEED & 1) != 0, AFB = (FEED & 2) != 0;
+  static_assert(FEED == 0 || (!CPLX && LA >= 0 && LB >= 0), "affine feed: real, fixed layout");
   constexpr int MT = Cfg::MT, NT8 = Cfg::NT8;
   constexpr int NCB = BN / 2, KCB = BK / 2;  // complex B tile extents
 
@@ -262,7 +322,7 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
 
   auto fill_ktab = [&](int kb) {
     // offsets of k-block kb into parity slot kb&1 (threads < BK)
-    if (tid < BK) {
+    if (!(AFA && AFB) && tid < BK) {
       int64_t kh = kbeg + (int64_t)kb * BK + tid, oa = -1, ob = -1;
       if (kb < nkb && kh < kend) {
         if (CPLX) {
@@ -277,12 +337,18 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
       else ktabB[(kb & 1) * BK + tid] = ob;
     }
   };
+  AffineFeed fA, fB;  // set once the row tables are visible
   auto issue = [&](int kb) {
     if (kb < nkb) {
       const int st = kb % STAGES;
-      load_tile<BM, BK, NT, LA>(sA + (size_t)st * Cfg::A_ELEMS, A, offAm,
-                                ktabA + (kb & 1) * BK, CPLX ? 2 : p.vecA, p.thrA, tid);
-      if (CPLX)
+      if constexpr (AFA)
+        load_affine<BM, BK, NT>(smem_u32(sA + (size_t)st * Cfg::A_ELEMS), fA, kb);
+      else
+        load_tile<BM, BK, NT, LA>(sA + (size_t)st * Cfg::A_ELEMS, A, offAm,
+                                  ktabA + (kb & 1) * BK, CPLX ? 2 : p.vecA, p.thrA, tid);
+      if constexpr (AFB)
+        load_affine<BN, BK, NT>(smem_u32(sB + (size_t)st * Cfg::B_ELEMS), fB, kb);
+      else if (CPLX)
         load_tile_cplx<NCB, KCB, Cfg::BC_PITCH, NT>(
             sB + (size_t)st * Cfg::B_ELEMS, B, offBn, ktabB + (kb & 1) * BK,
             p.thrB, tid);
@@ -298,6 +364,14 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
   if (!p.dA) asm volatile("griddepcontrol.wait;" ::: "memory");
   __syncthreads();
   QB_TRACE(1);
+  // affine operands: row 0 of the tile is in range (the planner proved
+  // whole tiles), its table entry is the tile's base
+  if constexpr (AFA)
+    fA = affine_setup<BM, BK, NT, LA == 1>(A + offAm[0] + kbeg / (p.vecA == 2 ? 2 : 1) * p.kstepA,
+                                           p.rstepA, p.kstepA, p.vecA, p.thrA, tid);
+  if constexpr (AFB)
+    fB = affine_setup<BN, BK, NT, LB == 1>(B + offBn[0] + kbeg / (p.vecB == 2 ? 2 : 1) * p.kstepB,
+                                           p.rstepB, p.kstepB, p.vecB, p.thrB, tid);
 #pragma unroll 1
   for (int s = 0; s < STAGES - 1; ++s) {
     issue(s);
@@ -330,7 +404,25 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
   }
 
   const bool early = ((warp >> 2) & 1) == 0 || (NT <= 128);
-  double af[MT][4], bf[NT8][2];
+  // fragments of k-step kk: A row block i, B column block j
+  auto load_af = [&](const double *tA, int kk, int i, double (&a)[4]) {
+    const int r = wm0 + i * 16 + g;
+    a[0] = tA[r * sAm + (kk + t) * sAk];
+    a[1] = tA[(r + 8) * sAm + (kk + t) * sAk];
+    a[2] = tA[r * sAm + (kk + t + 4) * sAk];
+    a[3] = tA[(r + 8) * sAm + (kk + t + 4) * sAk];
+  };
+  auto load_bf = [&](const double *tB, int kk, int j, double (&b)[2]) {
+    const int c = wn0 + j * 8 + g;
+    if (CPLX) {
+      const int kc0 = (kk + t) >> 1, kc1 = (kk + t + 4) >> 1, nc = c >> 1;
+      b[0] = flip_sign(tB[(kc0 * Cfg::BC_PITCH + nc) * 2 + comp], sgn_mask);
+      b[1] = flip_sign(tB[(kc1 * Cfg::BC_PITCH + nc) * 2 + comp], sgn_mask);
+    } else {
+      b[0] = tB[c * sBn + (kk + t) * sBk];
+      b[1] = tB[c * sBn + (kk + t + 4) * sBk];
+    }
+  };
 #pragma unroll 1
   for (int kb = 0; kb < nkb; ++kb) {
     cp_async_wait<STAGES - 2>();
@@ -343,33 +435,46 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
     fill_ktab(kb + STAGES);
     const double *tA = sA + (size_t)(kb % STAGES) * Cfg::A_ELEMS;
     const double *tB = sB + (size_t)(kb % STAGES) * Cfg::B_ELEMS;
+    if constexpr (FEED == 0) {
+      double af[MT][4], bf[NT8][2];
 #pragma unroll
-    for (int kk = 0; kk < BK; kk += 8) {
-      if (kk == 8 && !early) issue(kb + STAGES - 1);
+      for (int kk = 0; kk < BK; kk += 8) {
+        if (kk == 8 && !early) issue(kb + STAGES - 1);
 #pragma unroll
-      for (int i = 0; i < MT; ++i) {
-        const int r = wm0 + i * 16 + g;
-        af[i][0] = tA[r * sAm + (kk + t) * sAk];
-        af[i][1] = tA[(r + 8) * sAm + (kk + t) * sAk];
-        af[i][2] = tA[r * sAm + (kk + t + 4) * sAk];
-        af[i][3] = tA[(r + 8) * sAm + (kk + t + 4) * sAk];
+        for (int i = 0; i < MT; ++i) load_af(tA, kk, i, af[i]);
+#pragma unroll
+        for (int j = 0; j < NT8; ++j) load_bf(tB, kk, j, bf[j]);
+#pragma unroll
+        for (int i = 0; i < MT; ++i)
+#pragma unroll
+          for (int j = 0; j < NT8; ++j) dmma_16x8x8(acc[i][j], af[i], bf[j]);
       }
+    } else {
+      // fragment prefetch on the registers the tables no longer need: the B
+      // fragments of k-step kk+8 load while k-step kk's DMMAs issue, and
+      // A row block i of kk+8 as soon as its last DMMA of kk has issued.
+      // Same DMMAs, same order.
+      double af[MT][4], bf[2][NT8][2];
 #pragma unroll
-      for (int j = 0; j < NT8; ++j) {
-        const int c = wn0 + j * 8 + g;
-        if (CPLX) {
-          const int kc0 = (kk + t) >> 1, kc1 = (kk + t + 4) >> 1, nc = c >> 1;
-          bf[j][0] = flip_sign(tB[(kc0 * Cfg::BC_PITCH + nc) * 2 + comp], sgn_mask);
-          bf[j][1] = flip_sign(tB[(kc1 * Cfg::BC_PITCH + nc) * 2 + comp], sgn_mask);
-        } else {
-          bf[j][0] = tB[c * sBn + (kk + t) * sBk];
-          bf[j][1] = tB[c * sBn + (kk + t + 4) * sBk];
+      for (int i = 0; i < MT; ++i) load_af(tA, 0, i, af[i]);
+#pragma unroll
+      for (int j = 0; j < NT8; ++j) load_bf(tB, 0, j, bf[0][j]);
+#pragma unroll
+      for (int kk = 0; kk < BK; kk += 8) {
+        const int cur = (kk / 8) & 1;
+        const bool more = kk + 8 < BK;
+        if (kk == 8 && !early) issue(kb + STAGES - 1);
+        if (more) {
+#pragma unroll
+          for (int j = 0; j < NT8; ++j) load_bf(tB, kk + 8, j, bf[cur ^ 1][j]);
+        }
+#pragma unroll
+        for (int i = 0; i < MT; ++i) {
+#pragma unroll
+          for (int j = 0; j < NT8; ++j) dmma_16x8x8(acc[i][j], af[i], bf[cur][j]);
+          if (more) load_af(tA, kk + 8, i, af[i]);
         }
       }
-#pragma unroll
-      for (int i = 0; i < MT; ++i)
-#pragma unroll
-        for (int j = 0; j < NT8; ++j) dmma_16x8x8(acc[i][j], af[i], bf[j]);
     }
   }
   cp_async_wait<0>();
@@ -470,16 +575,30 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
 }
 
 template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
-          bool CPLX, int LA = -1, int LB = -1>
-__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
-    contract_f64_kernel(const __grid_constant__ ContractParams p) {
+          bool CPLX, int LA, int LB, int FEED>
+__device__ __forceinline__ void classic_grid(const ContractParams &p) {
   const int64_t Kh = CPLX ? 2 * p.K : p.K;
   const int ks = blockIdx.z;
   const int64_t kbeg = (int64_t)ks * p.k_per_split;  // in real-k units
   const int64_t kend = min(Kh, kbeg + p.k_per_split);
   SkSeg sk{0, (int)(blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z)), 0, 0, nullptr, nullptr, 0};
-  contract_tile<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB>(
+  contract_tile<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB, FEED>(
       p, blockIdx.x, blockIdx.y, ks, kbeg, kend, sk);
+}
+
+template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
+          bool CPLX, int LA = -1, int LB = -1>
+__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
+    contract_f64_kernel(const __grid_constant__ ContractParams p) {
+  classic_grid<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB, 0>(p);
+}
+
+// the large real tile with at least one operand on the affine feed
+template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES, int LA,
+          int LB, int FEED>
+__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
+    contract_f64_affine_kernel(const __grid_constant__ ContractParams p) {
+  classic_grid<BM, BN, BK, WARPS_M, WARPS_N, STAGES, false, LA, LB, FEED>(p);
 }
 
 // Stream-K: one persistent CTA per SM; the (tile, k-block) iteration space is
@@ -490,9 +609,8 @@ __global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
 // HEAD, processed last in its range, i.e. long after the tails were written)
 // adds them in a fixed order and runs the normal epilogue.
 template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
-          bool CPLX, int LA = -1, int LB = -1>
-__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
-    contract_f64_streamk_kernel(const __grid_constant__ ContractParams p) {
+          bool CPLX, int LA, int LB, int FEED>
+__device__ __forceinline__ void streamk_grid(const ContractParams &p) {
   const int64_t Kh = CPLX ? 2 * p.K : p.K;
   const int64_t nkbT = (Kh + BK - 1) / BK;
   const int64_t tiles = (int64_t)p.tiles_m * p.tiles_n;
@@ -521,11 +639,25 @@ __global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
       while (c < G && start(c) < (tile + 1) * nkbT) ++c;
       sk.peer1 = c;
     }
-    contract_tile<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB>(
+    contract_tile<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB, FEED>(
         p, (int)tile, 0, 0, kb0 * BK, min(Kh, kb1 * BK), sk);
     u += kb1 - kb0;
     __syncthreads();  // shared memory is reused by the next segment
   }
+}
+
+template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
+          bool CPLX, int LA = -1, int LB = -1>
+__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
+    contract_f64_streamk_kernel(const __grid_constant__ ContractParams p) {
+  streamk_grid<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB, 0>(p);
+}
+
+template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES, int LA,
+          int LB, int FEED>
+__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
+    contract_f64_affine_streamk_kernel(const __grid_constant__ ContractParams p) {
+  streamk_grid<BM, BN, BK, WARPS_M, WARPS_N, STAGES, false, LA, LB, FEED>(p);
 }
 
 // deterministic split-K reduction + strided scatter into C
@@ -589,11 +721,17 @@ static int launch_pdl(Kern kern, dim3 grid, int threads, size_t smem, cudaStream
   return 0;
 }
 
+// FEED != 0: the large real tile with affine operands (contract_tile)
 template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
-          bool CPLX, int LA = -1, int LB = -1>
+          bool CPLX, int LA = -1, int LB = -1, int FEED = 0>
 static int launch_cfg(const ContractParams &p, cudaStream_t st) {
   using Cfg = KernelCfg<BM, BN, BK, WARPS_M, WARPS_N, STAGES>;
-  auto kern = contract_f64_kernel<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB>;
+  auto kern = [] {
+    if constexpr (FEED == 0)
+      return contract_f64_kernel<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB>;
+    else
+      return contract_f64_affine_kernel<BM, BN, BK, WARPS_M, WARPS_N, STAGES, LA, LB, FEED>;
+  }();
   static bool attr_set = false;
   if (!attr_set) {
     QB_CUDA_CHECK(cudaFuncSetAttribute(
@@ -611,12 +749,18 @@ static int launch_cfg(const ContractParams &p, cudaStream_t st) {
 
 // The cfg-0 (large) tile: 128 x 128, BK 32, 3 stages, 8 warps.  Its real
 // kernels are specialised on the shared-memory layout of the operands
-// (a_kmajor / b_kmajor, plan.h); the route carries the choice.  The complex
-// kernel takes its layout at run time.
-template <bool CPLX, int LA, int LB>
+// (a_kmajor / b_kmajor, plan.h), which the route carries, and on which
+// operands the planner proved affine (feedA / feedB).  The complex kernel
+// takes its layout at run time and always gathers through the tables.
+template <bool CPLX, int LA, int LB, int FEED>
 static int launch_streamk_l(const PairPlan &plan, cudaStream_t st) {
   using Cfg = KernelCfg<128, 128, 32, 2, 4, 3>;
-  auto kern = contract_f64_streamk_kernel<128, 128, 32, 2, 4, 3, CPLX, LA, LB>;
+  auto kern = [] {
+    if constexpr (FEED == 0)
+      return contract_f64_streamk_kernel<128, 128, 32, 2, 4, 3, CPLX, LA, LB>;
+    else
+      return contract_f64_affine_streamk_kernel<128, 128, 32, 2, 4, 3, LA, LB, FEED>;
+  }();
   static bool attr_set = false;
   if (!attr_set) {
     QB_CUDA_CHECK(cudaFuncSetAttribute(
@@ -629,17 +773,37 @@ static int launch_streamk_l(const PairPlan &plan, cudaStream_t st) {
   return launch_pdl(kern, dim3(G), Cfg::NT, Cfg::SMEM, st, plan.p);
 }
 
+template <int LA, int LB>
+static int launch_streamk_feed(const PairPlan &plan, cudaStream_t st) {
+  switch (plan.p.feedA | plan.p.feedB << 1) {
+    case 0: return launch_streamk_l<false, LA, LB, 0>(plan, st);
+    case 1: return launch_streamk_l<false, LA, LB, 1>(plan, st);
+    case 2: return launch_streamk_l<false, LA, LB, 2>(plan, st);
+    default: return launch_streamk_l<false, LA, LB, 3>(plan, st);
+  }
+}
+
 template <bool CPLX>
 static int launch_streamk(const PairPlan &plan, const Route &r, cudaStream_t st) {
   if constexpr (CPLX) {
-    return launch_streamk_l<true, -1, -1>(plan, st);
+    return launch_streamk_l<true, -1, -1, 0>(plan, st);
   } else {
     switch (r.layout) {
-      case 0: return launch_streamk_l<false, 0, 0>(plan, st);
-      case 1: return launch_streamk_l<false, 0, 1>(plan, st);
-      case 2: return launch_streamk_l<false, 1, 0>(plan, st);
-      default: return launch_streamk_l<false, 1, 1>(plan, st);
+      case 0: return launch_streamk_feed<0, 0>(plan, st);
+      case 1: return launch_streamk_feed<0, 1>(plan, st);
+      case 2: return launch_streamk_feed<1, 0>(plan, st);
+      default: return launch_streamk_feed<1, 1>(plan, st);
     }
+  }
+}
+
+template <int LA, int LB>
+static int launch_cfg0_feed(const ContractParams &p, cudaStream_t st) {
+  switch (p.feedA | p.feedB << 1) {
+    case 0: return launch_cfg<128, 128, 32, 2, 4, 3, false, LA, LB, 0>(p, st);
+    case 1: return launch_cfg<128, 128, 32, 2, 4, 3, false, LA, LB, 1>(p, st);
+    case 2: return launch_cfg<128, 128, 32, 2, 4, 3, false, LA, LB, 2>(p, st);
+    default: return launch_cfg<128, 128, 32, 2, 4, 3, false, LA, LB, 3>(p, st);
   }
 }
 
@@ -649,10 +813,10 @@ static int launch_cfg0(const ContractParams &p, const Route &r, cudaStream_t st)
     return launch_cfg<128, 128, 32, 2, 4, 3, true>(p, st);
   } else {
     switch (r.layout) {
-      case 0: return launch_cfg<128, 128, 32, 2, 4, 3, false, 0, 0>(p, st);
-      case 1: return launch_cfg<128, 128, 32, 2, 4, 3, false, 0, 1>(p, st);
-      case 2: return launch_cfg<128, 128, 32, 2, 4, 3, false, 1, 0>(p, st);
-      default: return launch_cfg<128, 128, 32, 2, 4, 3, false, 1, 1>(p, st);
+      case 0: return launch_cfg0_feed<0, 0>(p, st);
+      case 1: return launch_cfg0_feed<0, 1>(p, st);
+      case 2: return launch_cfg0_feed<1, 0>(p, st);
+      default: return launch_cfg0_feed<1, 1>(p, st);
     }
   }
 }

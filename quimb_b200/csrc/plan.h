@@ -55,6 +55,12 @@ struct ContractParams {
   // fix-up + epilogue when the iteration space is cut into equal shares
   int *flags;
   int32_t sk_head;
+  // affine operand feed of the large real tile (affine_feed below): feedX = 1
+  // when every row of a tile and every k-block of operand X sits at
+  // tile_base + row_unit * rstepX + k_unit * kstepX (units: the operand's
+  // 16-byte pairs along rows / k, single elements otherwise)
+  int32_t feedA, feedB;
+  int64_t rstepA, kstepA, rstepB, kstepB;
   // tuning (QB_TRACE=1): per-CTA globaltimer stamps of the kernel phases
   unsigned long long *trace;
 };
@@ -121,6 +127,45 @@ constexpr int kNumTileCfgs = 5;
 constexpr double kDmmaFmaPerSmUs = 128.0 * 1980.0;
 
 inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// Affine feed of one operand of the large real tile (rows_tile x bk blocks).
+// It holds when
+//  - the leading modes of the operand's row group form one run that is
+//    jointly strided in this operand (stride[i] = stride[i-1] * ext[i-1])
+//    over a multiple of rows_tile rows: every tile's rows then sit at
+//    tile_base + r * stride[0];
+//  - its whole k group, counted in the operand's vector units (pairs of k when
+//    vec == 2), is one such run and K is a multiple of bk: a k-block's
+//    offsets are block_base + k_unit * kstep, and block_base advances by a
+//    constant per k-block.
+// The tile's thread walk (NT a multiple of both tile extents in units) keeps
+// every copy of a thread on base + i * step; contract_dmma.cu asserts that.
+// Steps are in doubles, per unit: rows in pairs when vec == 1.
+inline bool affine_feed(const ModeGroup &rows, const ModeGroup &k, bool k_second, int vec,
+                        int rows_tile, int bk, int64_t &rstep, int64_t &kstep) {
+  if (rows.n == 0 || k.n == 0) return false;
+  int64_t run = rows.ext[0];
+  for (int i = 1; i < rows.n && rows.s0[i] == rows.s0[i - 1] * rows.ext[i - 1]; ++i)
+    run *= rows.ext[i];
+  if (run % rows_tile) return false;
+  auto ks = [&](int i) { return k_second ? k.s1[i] : k.s0[i]; };
+  int64_t K = 1;
+  for (int i = 0; i < k.n; ++i) K *= k.ext[i];
+  if (K % bk) return false;
+  // the first k mode in units: extent / uk at stride uk (vec == 2 proved
+  // unit stride and an even extent); a mode of one pair drops out
+  const int uk = vec == 2 ? 2 : 1;
+  int first = 0;
+  int64_t e = k.ext[0] / uk, s = ks(0) * uk;
+  if (e == 1) { first = 1; e = k.ext[1]; s = ks(1); }  // k.n > 1: K >= bk > 2
+  kstep = s;
+  for (int i = first + 1; i < k.n; ++i) {
+    if (ks(i) != s * e) return false;
+    s = ks(i); e = k.ext[i];
+  }
+  rstep = rows.s0[0] * (vec == 1 ? 2 : 1);
+  return true;
+}
 
 // returns 0 or a negative argument-error code; fills plan
 inline int plan_pair(const qb_tensor_t *A, const int32_t *la,
@@ -355,6 +400,10 @@ inline int plan_pair(const qb_tensor_t *A, const int32_t *la,
   p.tiles_n = (int32_t)cdiv(N, tc.bn);
   p.splitk = best_split;
   p.k_per_split = best_kper;
+  if (cfg == 0 && !cplx) {
+    p.feedA = affine_feed(p.m, p.k, false, p.vecA, tc.bm, tc.bk, p.rstepA, p.kstepA);
+    p.feedB = affine_feed(p.n, p.k, true, p.vecB, tc.bn, tc.bk, p.rstepB, p.kstepB);
+  }
   // stream-K (large tile only): when the tile count leaves SMs idle in the
   // last wave, cut the (tile, k-block) space into one equal range per SM
   plan.streamk = 0;

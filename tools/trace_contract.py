@@ -1,7 +1,11 @@
 """Phase timing of the contraction kernel from its in-kernel %globaltimer stamps
-(QB_TRACE=1; GPU box only).  Runs the two launches of one MPS-norm site
-(chi=1024, d=2) back to back and prints, per launch, the median over CTAs of
-each phase and the gap between consecutive kernels.
+(QB_TRACE=1; GPU only).  Runs the two launches of one MPS-norm site
+(chi=1024, d=2, an "lrp" site viewed as (l, p, r), as bench.py contracts it)
+back to back and prints, per launch, the median over CTAs of each phase and
+the gap between consecutive kernels.  The CTA count of each launch comes from
+its route (the stream-K grid is one CTA per SM).
+
+  python tools/trace_contract.py [--out trace.json]
 
 phases: 0 entry, 1 tables done, 2 prologue issued, 3 first tile landed,
         4 main loop done, 5 stream-K fix-up done, 6 stores issued
@@ -29,7 +33,7 @@ def read_trace():
     return np.frombuffer(buf, dtype=np.uint64).reshape(16, 8192).copy()
 
 
-def analyse(slot, G=148):
+def analyse(slot, G):
     t = slot[: G * 32].reshape(G, 4, 8).astype(np.int64)
     out = {}
     seg_used = (t[:, :, 0] > 0)
@@ -58,7 +62,9 @@ def main():
     dev = torch.device("cuda:0")
     chi, d = 1024, 2
     g = torch.Generator(device=dev); g.manual_seed(0)
-    A = qb.asarray(torch.randn((chi, d, chi), dtype=torch.float64, device=dev, generator=g))
+    # lrp storage, (l, p, r) view: strides (chi * d, 1, d)
+    A = mps.site_lpr(torch.randn((chi, chi, d), dtype=torch.float64, device=dev, generator=g),
+                     "lrp", 1, 3)
     E = qb.asarray(torch.randn((chi, chi), dtype=torch.float64, device=dev, generator=g))
     for _ in range(3):
         E2 = mps.norm_step(E, A)
@@ -72,17 +78,34 @@ def main():
     print("4 sites:", e0.elapsed_time(e1) * 1e3, "us")
     tr = read_trace()
     used = [i for i in range(16) if tr[i].any()]
+    # the CTAs of each launch: ket E . A, then bra conj(A) . T
+    LB, L, P, R, RB = 0, 1, 2, 3, 4
+    T = torch.empty((chi, d, chi), dtype=torch.float64, device=dev)
+    a = A.t
+    grids = []
+    for (x, lx, y, ly, z, lz) in ((E.t, [LB, L], a, [L, P, R], T, [LB, P, R]),
+                                  (a, [LB, P, RB], T, [LB, P, R], E2.t, [RB, R])):
+        args = (list(x.shape), list(x.stride()), lx, list(y.shape), list(y.stride()), ly,
+                list(z.shape), list(z.stride()), lz)
+        ptrs = (x.data_ptr(), y.data_ptr(), z.data_ptr())
+        r = qb.route_pair(*args, ptrs=ptrs)
+        f = qb.feed_pair(*args, ptrs=ptrs)
+        tiles = (x.shape[0] // 128) * (z.numel() // x.shape[0] // 128) if r["streamk"] == 0 else 0
+        grids.append((r["streamk"] or tiles, r, f))
+        print(json.dumps({"route": r, "feed": f}))
     res = []
-    for i in used:
-        res.append(analyse(tr[i]))
+    for n, i in enumerate(used):
+        G, r, f = grids[n % 2]
+        res.append({"kind": r["kind"], "layout": r["layout"], "ctas": G, "feed": f,
+                    **analyse(tr[i], G)})
     res.sort(key=lambda r: r["start_ns"])
     for k, r in enumerate(res):
         gap = (r["start_ns"] - res[k - 1]["end_ns"]) / 1e3 if k else None
         print(json.dumps({"launch": k, "gap_before_us": gap, **{a: b for a, b in r.items()
                                                                if a not in ("start_ns", "end_ns")}}))
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/trace_contract.json", "w") as fh:
-        json.dump(res, fh, indent=1)
+    if "--out" in sys.argv:
+        with open(sys.argv[sys.argv.index("--out") + 1], "w") as fh:
+            json.dump(res, fh, indent=1)
 
 
 if __name__ == "__main__":
