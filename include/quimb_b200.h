@@ -26,6 +26,9 @@
  *                            MatrixProductState.sample_configuration,
  *                            quimb/tensor/tn1d/core.py:3871-3990, for a whole
  *                            batch of samples at once
+ *   qb_rdm_reduce         <- the final contraction of
+ *                            MatrixProductState.partial_trace_to_dense_canonical
+ *                            and of the local expectations, core.py:2827-3087
  *
  * Conventions
  *   - plain C, no C++/torch types; device pointers are borrowed, never freed
@@ -367,6 +370,33 @@ int qb_svals_to_keep(const double *s, int64_t n, double cutoff,
 int qb_sample_select(int dtype, int64_t C, int64_t d, int64_t r, const void *W,
                      const double *u, int64_t ldu, int64_t *config, int64_t ldc,
                      double *omega, void *V, void *stream);
+
+/* ---- MPS reduced density matrices -------------------------------------- */
+/*
+ * The reduction that ends every reduced density matrix of an MPS
+ * (partial_trace_to_dense_canonical / local expectations,
+ * quimb/tensor/tn1d/core.py:2827-3087):
+ *   out[m, n] = sum_{a < n1, b < n2} U[a, m, b] * conj(V[a, n, b])
+ * U and V are strided views (strides in elements, any sign; permuted views
+ * need no copy) of dtype QB_F64 (conj is the identity) or QB_C128 (16-byte
+ * aligned); out is M x N, contiguous.  Accumulation is fp64 (pairs of fp64
+ * for complex); NaN and Inf propagate.  When U == V with equal strides each
+ * element is loaded once.  At most two launches on `stream` (partials over
+ * fixed K-tiles, then a fixed-order reduction), no allocation and no host
+ * synchronisation, so the call can be captured in a graph.  The grid and the
+ * summation order depend on (n1, M, N, n2) only: the same input gives the
+ * same bits on any device or stream, and whether or not U aliases V.
+ * 1 <= M, N <= 64 (-2), n1, n2 >= 1 (-3), U, V, out or a stride array null
+ * or misaligned (-4), workspace smaller than qb_rdm_workspace (-6), any
+ * other dtype (-1); nothing is launched when a call is rejected.
+ * qb_rdm_workspace returns the bytes needed (0 for a single block) or the
+ * same negative codes.
+ */
+int64_t qb_rdm_workspace(int64_t n1, int64_t M, int64_t N, int64_t n2);
+int qb_rdm_reduce(int dtype, int64_t n1, int64_t M, int64_t N, int64_t n2,
+                  const void *U, const int64_t ustride[3],
+                  const void *V, const int64_t vstride[3],
+                  void *out, void *workspace, int64_t ws_bytes, void *stream);
 
 /* ---- device queries / microbenchmarks ---------------------------------- */
 /* ------------------------------------------------------------------------

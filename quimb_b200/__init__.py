@@ -40,6 +40,13 @@ from .tebd import (TEBD, LocalHam1D, gate_split, gate_with_auto_swap,  # noqa: F
 from .boundary import (BoundaryContractor2D, contract_boundary,  # noqa: F401
                        contract_boundary_two_sided, peps_norm_tensors)
 from .dmrg import DMRG1, DMRG2  # noqa: F401
+from . import observables  # noqa: F401
+from .observables import (mps_calc_current_orthog_center, mps_canonicalize,  # noqa: F401
+                          mps_compute_local_expectation, mps_correlation,
+                          mps_count_canonized, mps_entropy,
+                          mps_local_expectation_canonical, mps_magnetization,
+                          mps_partial_trace_to_dense_canonical, mps_schmidt_gap,
+                          mps_schmidt_values, mps_singular_values)
 from .compressed import contract_compressed, path_to_sequence  # noqa: F401
 from .integration import register_with_quimb  # noqa: F401
 

@@ -619,6 +619,11 @@ def mps_compress(sites, form=None, **compress_opts):
 def mps_overlap(bra, ket):
     """<bra|ket> of two (l, p, r) MPS with matching physical dimensions: two
     launches per site, the bra conjugated on load."""
+    return mps_overlap_array(bra, ket).item()
+
+
+def mps_overlap_array(bra, ket):
+    """:func:`mps_overlap` as a 0-d device Array (nothing read back)."""
     E = None
     for A, B in zip(bra, ket):
         if E is None:
@@ -629,7 +634,7 @@ def mps_overlap(bra, ket):
             A, B, E = A.astype(dt, copy=False), B.astype(dt, copy=False), E.astype(dt, copy=False)
         T = contract_pair(E.t, [0, 1], B.t, [1, 2, 3], [0, 2, 3], conj_a=E.cj, conj_b=B.cj)
         E = Array(contract_pair(A.t, [0, 2, 4], T, [0, 2, 3], [4, 3], conj_a=not A.cj))
-    return E.reshape(()).item()
+    return E.reshape(())
 
 
 def mps_add(a, b):
