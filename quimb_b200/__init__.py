@@ -47,6 +47,8 @@ from .observables import (mps_calc_current_orthog_center, mps_canonicalize,  # n
                           mps_local_expectation_canonical, mps_magnetization,
                           mps_partial_trace_to_dense_canonical, mps_schmidt_gap,
                           mps_schmidt_values, mps_singular_values)
+from . import mpo_compress  # noqa: F401
+from .mpo_compress import mps_gate_with_mpo  # noqa: F401
 from .compressed import contract_compressed, path_to_sequence  # noqa: F401
 from .integration import register_with_quimb  # noqa: F401
 
