@@ -49,6 +49,8 @@ from .observables import (mps_calc_current_orthog_center, mps_canonicalize,  # n
                           mps_schmidt_values, mps_singular_values)
 from . import mpo_compress  # noqa: F401
 from .mpo_compress import mps_gate_with_mpo  # noqa: F401
+from . import fit  # noqa: F401
+from .fit import mps_fit, mps_gate_with_mpo_fit  # noqa: F401
 from .compressed import contract_compressed, path_to_sequence  # noqa: F401
 from .integration import register_with_quimb  # noqa: F401
 
