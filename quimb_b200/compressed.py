@@ -1,6 +1,6 @@
 """Compressed contraction along a given contraction sequence on the device:
 the array-level mirror of ``TensorNetwork._contract_compressed_tid_sequence``
-(quimb/tensor/tensor_core.py:8560-8780) behind ``contract_compressed``
+(quimb/tensor/tensor_core.py:8429-8718) behind ``contract_compressed``
 (:8839-9080), SURVEY.md 8(f) rank 3.
 
 What is mirrored is the reference's control flow for ``compress_mode='basic'``
@@ -75,16 +75,23 @@ class _Network:
         return n
 
     def strip_exponent(self, tid, value):
-        """Rescale tensor ``tid`` to largest magnitude ``value`` (True: 1.0),
-        accumulating log10 of the factor (``TensorNetwork.strip_exponent``)."""
+        """Rescale tensor ``tid`` to Frobenius norm ``value`` (True: 1.0),
+        accumulating log10 of the factor (``TensorNetwork.strip_exponent``,
+        tensor_core.py:10809-10841).  The norm sets the scale the next
+        compression's absolute cutoffs see, so it must be the reference's.
+        A zero or non-finite norm leaves the tensor as it is (DESIGN 4.7)."""
         t = self.t[tid]
         target = 1.0 if value is True else float(value)
-        mx = float(ops.max(ops.abs(t.data)).item())
-        if mx == 0.0 or not math.isfinite(mx):
+        nrm = _norm(t.data)
+        if nrm == 0.0 or not math.isfinite(nrm):
             return
-        f = mx / target
+        f = nrm / target
         t.data = t.data / f
         self.exponent += math.log10(f)
+
+
+def _norm(data):
+    return float(ops.norm_fro(data).item()) if data.size else 0.0
 
 
 def _fuse_squeeze(net, a, b):
@@ -125,7 +132,7 @@ def path_to_sequence(path, n):
 def contract_compressed(arrays, inputs, output, seq, max_bond=None, cutoff=1e-10,
                         tree_gauge_distance=0, compress_mode="basic", compress_late=True,
                         compress_min_size=None, compress_span=False, compress_matrices=True,
-                        compress_exclude=None, compress_opts=None, equalize_norms=False,
+                        compress_exclude=None, compress_opts=None, equalize_norms="auto",
                         strip_exponent=False, gauges=None, info=None):
     """Contract the network ``(arrays, inputs) -> output`` along ``seq``,
     compressing bonds larger than ``max_bond`` on the way.
@@ -137,6 +144,9 @@ def contract_compressed(arrays, inputs, output, seq, max_bond=None, cutoff=1e-10
     Returns a device Array (0-d for a scalar network); with
     ``strip_exponent=True`` the pair ``(mantissa, log10 exponent)``.
     ``info`` (dict) receives ``max_bond_seen`` and ``n_compress``.
+    ``equalize_norms='auto'`` (the reference's default) follows
+    ``strip_exponent``: tensors are then divided by their Frobenius norm after
+    every contraction and compression.
     """
     if tree_gauge_distance not in (0, None) or gauges not in (None, False):
         raise NotImplementedError(
@@ -237,10 +247,11 @@ def contract_compressed(arrays, inputs, output, seq, max_bond=None, cutoff=1e-10
         info.update(stats)
     data = res.data
     if strip_exponent:
-        mx = float(ops.max(ops.abs(data)).item()) if data.size else 1.0
-        if mx > 0.0 and math.isfinite(mx):
-            data = data / mx
-            net.exponent += math.log10(mx)
+        # maybe_unwrap (tensor_core.py:1891-1894): mantissa of unit Frobenius norm
+        nrm = _norm(data)
+        if nrm > 0.0 and math.isfinite(nrm):
+            data = data / nrm
+            net.exponent += math.log10(nrm)
         return data, net.exponent
     if net.exponent:
         data = data * (10.0 ** net.exponent)

@@ -69,3 +69,31 @@ def test_contract_compressed_paths_and_errors(golden_compressed):
     with pytest.raises(NotImplementedError):
         qb.contract_compressed(arrays, m["inputs"], m["output"], seq, max_bond=4,
                                tree_gauge_distance=1)
+
+
+@pytest.mark.parametrize("name", ["peps33_open", "peps34_open_c", "flat55", "reg12"])
+def test_contract_compressed_rescaling_matches_reference(name):
+    """tests/golden/compressed2.* (oracle/make_golden_compressed2.py): the
+    reference divides tensors by their Frobenius norm, so with equalize_norms
+    an absolute ('abs', 'sum2') cutoff keeps what that norm decides, and a
+    stripped mantissa of an open output has unit Frobenius norm.  Every cut
+    of these runs lies at a relative gap >= 1e-6, so the kept ranks and the
+    value are the reference's to rounding."""
+    data, meta = load_golden("compressed2")
+    m = meta[name]
+    arrays = [qb.asarray(data[f"{name}__t{k}"]) for k in range(len(m["inputs"]))]
+    for run in m["runs"]:
+        kw = dict(run["kw"])
+        if "cutoff_mode" in kw:
+            kw["compress_opts"] = {"cutoff_mode": kw.pop("cutoff_mode")}
+        info = {}
+        out = qb.contract_compressed(arrays, m["inputs"], m["output"], m["seq"], info=info, **kw)
+        ref = data[run["key"]]
+        assert (info["n_compress"], info["max_bond_seen"]) == (
+            run["n_compress"], run["max_bond_seen"]), (name, kw)
+        if run["exponent"] is not None:
+            out, ex = out
+            assert abs(ex - run["exponent"]) <= 1e-10, (name, kw, ex, run["exponent"])
+        got = out.to_numpy()
+        assert got.shape == ref.shape
+        assert np.abs(got - ref).max() <= 1e-9 * np.abs(ref).max(), (name, kw)
