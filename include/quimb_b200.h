@@ -29,6 +29,9 @@
  *   qb_rdm_reduce         <- the final contraction of
  *                            MatrixProductState.partial_trace_to_dense_canonical
  *                            and of the local expectations, core.py:2827-3087
+ *   qb_sketch_env         <- the noise-sketched left environments of
+ *                            tensor_network_1d_compress_src,
+ *                            quimb/tensor/tn1d/compress.py:1787-1826
  *
  * Conventions
  *   - plain C, no C++/torch types; device pointers are borrowed, never freed
@@ -397,6 +400,29 @@ int qb_rdm_reduce(int dtype, int64_t n1, int64_t M, int64_t N, int64_t n2,
                   const void *U, const int64_t ustride[3],
                   const void *V, const int64_t vstride[3],
                   void *out, void *workspace, int64_t ws_bytes, void *stream);
+
+/* ---- sketched left environments of successive randomized compression --- */
+/*
+ * The first half of one left-environment step of SRC on an MPS / MPO ladder
+ * (tensor_network_1d_compress_src, quimb/tensor/tn1d/compress.py:1653-1840):
+ *   H[B, a, u, p] = sum_{v < nv, o < no} LE[B, a, v] W[v, u, o, p] Om[B, o]
+ * with nB samples B; the step ends with LE'[B, b, u] = sum H[B, a, u, p]
+ * A[a, p, b], one ordinary contraction.  Every operand is a strided view
+ * (strides in elements, any sign, 0 allowed on the inputs; H must not
+ * overlap an input), all of one dtype: QB_F32, QB_F64, QB_C64 or QB_C128;
+ * no conjugation.  Single precision is accumulated in fp64 and rounded once.
+ * Exactly one launch on `stream`, no allocation, no host synchronisation.
+ * Every output is a sum over v in order of products with the sum over o in
+ * order, and the grid depends on (nB, na, nu np) alone, so the same input
+ * gives the same bits on any device or stream; NaN and Inf propagate.
+ * Unknown dtype (-1), an extent below 1 (-2), a pointer or stride array null
+ * or misaligned (-3), a grid of more than 2^31 - 1 blocks (-4); nothing is
+ * launched when a call is rejected.
+ */
+int qb_sketch_env(int dtype, int64_t nB, int64_t na, int64_t nv, int64_t nu, int64_t no,
+                  int64_t np, const void *LE, const int64_t lestride[3], const void *W,
+                  const int64_t wstride[4], const void *Om, const int64_t omstride[2],
+                  void *H, const int64_t hstride[4], void *stream);
 
 /* ---- device queries / microbenchmarks ---------------------------------- */
 /* ------------------------------------------------------------------------

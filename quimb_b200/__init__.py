@@ -51,6 +51,8 @@ from . import mpo_compress  # noqa: F401
 from .mpo_compress import mps_gate_with_mpo  # noqa: F401
 from . import fit  # noqa: F401
 from .fit import mps_fit, mps_gate_with_mpo_fit  # noqa: F401
+from . import successive  # noqa: F401
+from .successive import mps_gate_with_mpo_successive  # noqa: F401
 from .compressed import contract_compressed, path_to_sequence  # noqa: F401
 from .integration import register_with_quimb  # noqa: F401
 
@@ -70,6 +72,12 @@ def _random_array(shape, dist="normal", dtype="float64", rng=None, seed=None,
     tn1d/compress.py:1283): values drawn on the host from a numpy Generator
     (``rng`` / ``seed``: reproducible, same stream as the numpy backend) and
     placed on the device."""
+    return asarray(_random_host(shape, dist, dtype, rng, seed, loc, scale))  # noqa: F405
+
+
+def _random_host(shape, dist="normal", dtype="float64", rng=None, seed=None, loc=0.0,
+                scale=1.0):
+    """The host draw of ``random.array``: a numpy array, not yet uploaded."""
     import numpy as _np
     if rng is None:
         if seed is None:
@@ -99,7 +107,7 @@ def _random_array(shape, dist="normal", dtype="float64", rng=None, seed=None,
     if dt.kind == "c":
         x = (x + 1j * draw()) / 2 ** 0.5 if dist != "rademacher" else x + 0j
     x = x * scale + loc
-    return asarray(_np.asarray(x, dtype=dt))  # noqa: F405
+    return _np.asarray(x, dtype=dt)
 
 
 class _DeviceGenerator:

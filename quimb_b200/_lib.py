@@ -106,6 +106,8 @@ def load(build_if_missing=True):
     sig("qb_sample_select", ci, [ci, i64, i64, i64, vp, vp, i64, vp, i64, vp, vp, vp])
     sig("qb_rdm_workspace", i64, [i64, i64, i64, i64])
     sig("qb_rdm_reduce", ci, [ci, i64, i64, i64, i64, vp, P(i64), vp, P(i64), vp, vp, i64, vp])
+    sig("qb_sketch_env", ci, [ci, i64, i64, i64, i64, i64, i64, vp, P(i64), vp, P(i64), vp,
+                              P(i64), vp, P(i64), vp])
     for name, res, args in (
         ("qb_qr_stab", ci, [ci, i64, i64, vp, vp, vp, ci, vp, ctypes.c_size_t, vp]),
         ("qb_qr_workspace", i64, [ci, i64, i64]),
