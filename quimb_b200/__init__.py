@@ -53,6 +53,9 @@ from . import fit  # noqa: F401
 from .fit import mps_fit, mps_gate_with_mpo_fit  # noqa: F401
 from . import successive  # noqa: F401
 from .successive import mps_gate_with_mpo_successive  # noqa: F401
+from . import nonlocal_gates  # noqa: F401
+from .nonlocal_gates import (mpo_from_dense, mps_gate_controlled,  # noqa: F401
+                             mps_gate_nonlocal, mps_gate_with_submpo)
 from .compressed import contract_compressed, path_to_sequence  # noqa: F401
 from .integration import register_with_quimb  # noqa: F401
 

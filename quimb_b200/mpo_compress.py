@@ -106,14 +106,21 @@ def _prepare(sites, mpo, mpo_shape, transpose):
 def _flip(A, W):
     """The ladder read from the other end."""
     return ([a.transpose(2, 1, 0) for a in reversed(A)],
-            [w.transpose(1, 0, 2, 3) for w in reversed(W)])
+            [_flip_w(w) for w in reversed(W)])
+
+
+def _flip_w(w):
+    if isinstance(w, int):
+        return w
+    return w.transpose(1, 0) if w.ndim == 2 else w.transpose(1, 0, 2, 3)
 
 
 def _flip_mps(A):
     return [a.transpose(2, 1, 0) for a in reversed(A)]
 
 
-def ladder_tree_span(L, bond_a, bond_w, phys, root):
+def ladder_tree_span(L, bond_a, bond_w, phys, root, gaps=(), open_ends=(False, False),
+                     rung_between=False):
     """``get_tree_span`` (networking.py:196-356, defaults: weight_bonds,
     ndim_sort 'max', distance_sort 'min', inwards) of the MPS / MPO ladder
     fanning out from site ``root``: the ordered merges ``(n1, n2)``, node
@@ -122,18 +129,35 @@ def ladder_tree_span(L, bond_a, bond_w, phys, root):
     Models the network ``gate_with_mpo`` builds: MPS tensors first, then MPO
     tensors; index orders 'lrp' and 'lrud' without the end sites' outer
     bonds.  ``bond_a[i]`` / ``bond_w[i]`` are the bonds (i, i + 1) of the two
-    layers, ``phys[i]`` the rung of site i."""
+    layers, ``phys[i]`` the rung of site i.
+
+    The sub-range network of ``gate_with_submpo`` (tn1d/core.py:2339-2442)
+    differs in three ways: sites in ``gaps`` carry a two-index identity on
+    the MPO layer instead of an MPO tensor (no rung; enforce_1d_like,
+    compress.py:38-125), ``open_ends`` marks MPS end tensors that keep their
+    bond to the rest of the chain as an outer index, and with
+    ``rung_between`` the MPO tensors list their rung between their left and
+    right bonds (the index order of ``MatrixProductOperator.from_dense``)."""
+    gaps = frozenset(gaps)
+
     def ndim(n):
         i = n % L
-        return (3 if n < L else 4) - (i == 0) - (i == L - 1)
+        if n < L:
+            return 3 - (i == 0 and not open_ends[0]) - (i == L - 1 and not open_ends[1])
+        if i in gaps:
+            return 2
+        return 4 - (i == 0) - (i == L - 1)
 
     def neighbours(n):
         i, off = n % L, (0 if n < L else L)
         out = [off + i - 1] if i > 0 else []
+        rung = [] if i in gaps else [n + L if n < L else n - L]
+        if rung_between and n >= L:
+            out += rung
+            rung = []
         if i < L - 1:
             out.append(off + i + 1)
-        out.append(n + L if n < L else n - L)
-        return out
+        return out + rung
 
     def size(n1, n2):
         if abs(n1 - n2) == L:
@@ -178,25 +202,76 @@ def _ladder_inds(L, n):
     return (("w", i - 1), ("w", i), ("o", i), ("p", i))
 
 
-def _canonize_around(A, W, root):
+def _ladder_inds_gap(L, n, W):
+    i = n % L
+    if n >= L and W[i].ndim == 2:
+        return (("w", i - 1), ("w", i))
+    return _ladder_inds(L, n)
+
+
+def _canonize_around(A, W, root, **span_opts):
     """``canonize_around_(site root)`` of the ladder: the QR moves of the
     spanning tree, inwards (tensor_canonize_bond, absorb='right'), on new
-    lists."""
+    lists.  A gap site of a sub-range ladder (``W[i]`` an int, the size of
+    the bond passing it) enters as the identity matrix the reference threads
+    through it; the gauge generally leaves a full matrix there."""
     L = len(A)
+    gaps = [i for i, w in enumerate(W) if isinstance(w, int)]
+    W = [ops.eye(w, dtype=A[0].dtype, device=A[0].device) if isinstance(w, int) else w
+         for w in W]
     T = list(A) + list(W)
     seq = ladder_tree_span(L, [a.shape[2] for a in A[:-1]], [w.shape[1] for w in W[:-1]],
-                           [a.shape[1] for a in A], root)
+                           [a.shape[1] for a in A], root, gaps=gaps, **span_opts)
     for n1, n2 in seq:
-        T[n1], T[n2] = tensor_canonize_bond(T[n1], _ladder_inds(L, n1), T[n2],
-                                            _ladder_inds(L, n2), absorb="right")
+        T[n1], T[n2] = tensor_canonize_bond(T[n1], _ladder_inds_gap(L, n1, W), T[n2],
+                                            _ladder_inds_gap(L, n2, W), absorb="right")
     return T[:L], T[L:]
 
 
 def _product_site(a, w):
-    """A[a, p, b] W[w, v, o, p] -> site[(a w), o, (b v)]."""
+    """A[a, p, b] W[w, v, o, p] -> site[(a w), o, (b v)]; at a gap site
+    (``w`` the int size of the MPO bond passing it) the index expansion
+    A[a, p, b] delta[w, v], placed without a contraction."""
+    if isinstance(w, int):
+        return _expand_site(a, w)
     t = _cp(a, [0, 1, 2], w, [3, 4, 5, 1], [0, 3, 5, 2, 4])
     l, wl, o, r, wr = t.shape
     return t.reshape(l * wl, o, r * wr)
+
+
+def _expand_site(a, D):
+    """site[(a w), p, (b v)] = A[a, p, b] delta[w, v]: one permute launch
+    copies A, broadcast over w, onto the (w, v) diagonal of a zeroed buffer."""
+    from . import _lib
+    x = a.t
+    l, p, r = x.shape
+    out = ops.zeros((l, D, p, r, D), dtype=a.dtype, device=a.device).t
+    if out.numel():
+        src = x.unsqueeze(-1).expand(l, p, r, D)
+        dst = out.diagonal(dim1=1, dim2=4)
+        rc = _lib.load().qb_permute(_lib.desc(src), _lib.desc(dst), int(a.cj),
+                                    _lib.stream_ptr())
+        _lib.check(rc, "qb_permute")
+    return Array(out.reshape(l * D, p, r * D))
+
+
+def _seed(A):
+    """The right boundary of a contraction carried in from the right:
+    delta[b, k] over the ladder's last MPS bond, with a size-1 MPO bond
+    (ones((1, 1, 1)) when that bond is closed)."""
+    r = A[-1].shape[2]
+    return Array(ops.eye(r, dtype=A[0].dtype, device=A[0].device).t.reshape(r, 1, r))
+
+
+def _carry(a, w, R):
+    """C[a, w, o, k] = sum R[b, v, k] A[a, p, b] W[w, v, o, p], with W the
+    identity at a gap site (one launch) or a gauged gap matrix W[w, v]."""
+    if isinstance(w, int):
+        return _cp(a, [0, 1, 2], R, [2, 3, 4], [0, 3, 1, 4])
+    T = _cp(a, [0, 1, 2], R, [2, 3, 4], [0, 1, 3, 4])                  # [a, p, v, k]
+    if w.ndim == 2:
+        return _cp(T, [0, 1, 3, 4], w, [5, 3], [0, 5, 1, 4])
+    return _cp(T, [0, 1, 3, 4], w, [5, 3, 6, 1], [0, 5, 6, 4])
 
 
 # ------------------------------------------------------------------ methods ---
@@ -220,24 +295,29 @@ def _direct_sweep(out, opts):
         tebd.right_compress_site(out, i, **opts)
 
 
-def _zipup(A, W, canonize, rev, opts):
+def _zipup(A, W, canonize, rev, opts, span_opts=None):
     """compress.py:668-864 over the ladder read from the right (from the left
     when ``rev``): pseudo-canonical gauge around the starting end, then carry
     U s leftwards, splitting C = (U s) A W at every site (absorb='left').
-    The result is right-canonical in the direction of the sweep."""
+    The result is right-canonical in the direction of the sweep.
+
+    The ladder may be a sub-range of a longer chain: the MPS end bonds are
+    then open outer indices (the first product keeps its left bond, the
+    carry starts from delta over the last right bond), a gap site (``W[i]``
+    an int) carries an identity, and ``span_opts`` describe the sub-range
+    network to :func:`ladder_tree_span`."""
     L = len(A)
     opts = dict(opts)
     opts.setdefault("absorb", "left")
     if canonize:
-        A, W = _canonize_around(A, W, 0 if rev else L - 1)
+        A, W = _canonize_around(A, W, 0 if rev else L - 1, **(span_opts or {}))
     if rev:
         A, W = _flip(A, W)
     ts = [None] * L
-    Us = Array(ops.ones((1, 1, 1), dtype=A[0].dtype, device=A[0].device).t)
+    Us = _seed(A)
     for i in range(L - 1, -1, -1):
         # C[a, w, o, k] = sum Us[b, v, k] A[a, p, b] W[w, v, o, p]
-        T = _cp(A[i], [0, 1, 2], Us, [2, 3, 4], [0, 1, 3, 4])
-        C = _cp(T, [0, 1, 3, 4], W[i], [5, 3, 6, 1], [0, 5, 6, 4])
+        C = _carry(A[i], W[i], Us)
         la, lw, o, k = C.shape
         if i == 0:
             ts[0] = C.reshape(la * lw, o, k)
@@ -254,7 +334,9 @@ def _dm(A, W, opts):
     then from the right one reduced density matrix per site, split by
     ``eigh``; U^dagger folded into the ket's right environment.  The bra's
     environment is the conjugate of the ket's and is never formed: it enters
-    every contraction as a conjugation flag."""
+    every contraction as a conjugation flag.  On a sub-range ladder (see
+    :func:`_zipup`) the first environment traces over the open left bond and
+    the right environment starts from delta over the open right bond."""
     L = len(A)
     opts = dict(opts)
     opts.setdefault("method", "eigh")
@@ -266,10 +348,13 @@ def _dm(A, W, opts):
     for i in range(L - 1):
         a, w = A[i], W[i]
         if E is None:
-            T = _product_site(a, w)
-            _, o, r = T.shape
-            T = T.reshape(o, a.shape[2], w.shape[1])
+            # the trace runs over the open left bond too, when there is one
+            T = _product_site(a, w).reshape(-1, a.shape[2], w.shape[1])
             E = _cp(T, [0, 1, 2], T.conj(), [0, 3, 4], [1, 2, 3, 4])
+        elif isinstance(w, int):
+            # gap site: the identities of the two layers only relabel w
+            X = _cp(E, [0, 1, 2, 3], a, [0, 4, 5], [1, 2, 3, 4, 5])             # [w, a', w', p, b]
+            E = _cp(X, [1, 2, 3, 4, 5], a.conj(), [2, 4, 10], [5, 1, 10, 3])   # [b, w, b', w']
         else:
             X = _cp(E, [0, 1, 2, 3], a, [0, 4, 5], [1, 2, 3, 4, 5])             # [w, a', w', p, b]
             X = _cp(X, [1, 2, 3, 4, 5], W[i], [1, 6, 7, 4], [2, 3, 5, 6, 7])    # [a', w', b, v, o]
@@ -277,11 +362,10 @@ def _dm(A, W, opts):
             E = _cp(X, [2, 5, 6, 9, 8], a.conj(), [2, 9, 10], [5, 6, 10, 8])   # [b, v, b', v']
         envs[i + 1] = E
     out = [None] * L
-    R = Array(ops.ones((1, 1, 1), dtype=A[0].dtype, device=A[0].device).t)   # R[b, v, k]
+    R = _seed(A)                                                             # R[b, v, k]
     for i in range(L - 1, -1, -1):
         # Y[a, w, o, k] = sum A[a, p, b] W[w, v, o, p] R[b, v, k]: the ket side
-        T = _cp(A[i], [0, 1, 2], R, [2, 3, 4], [0, 1, 3, 4])
-        Y = _cp(T, [0, 1, 3, 4], W[i], [5, 3, 6, 1], [0, 5, 6, 4])
+        Y = _carry(A[i], W[i], R)
         la, lw, o, k = Y.shape
         if i == 0:
             out[0] = Y.reshape(la * lw, o, k)

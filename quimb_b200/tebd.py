@@ -377,23 +377,70 @@ def mps_zero_state(n, d=2, dtype="complex128"):
     return out
 
 
-def apply_circuit(sites, gates, **compress_opts):
+def apply_circuit(sites, gates, contract="swap+split", **compress_opts):
     """Run a gate list on an MPS in place, the way quimb's ``CircuitMPS`` does
     (quimb/tensor/circuit/mps.py): one-qubit gates are contracted into their
     site, two-qubit gates go through ``gate_with_auto_swap`` (swap to
     adjacency, canonicalise, contract + truncated split, swap back).
 
     ``gates``: iterable of ``(G, (i,))`` or ``(G, (i, j))`` with ``G`` a
-    (2, 2) / (4, 4) or (2, 2, 2, 2) array, index order (out..., in...)."""
+    (2, 2) / (4, 4) or (2, 2, 2, 2) array, index order (out..., in...).
+
+    ``contract`` chooses how gates on several sites are applied, as
+    ``gate_contract`` does (tn1d/core.py:214-246):
+
+      'swap+split'  (default) two-site gates only, by ``gate_with_auto_swap``
+      'auto-mps'    two-site gates by ``gate_with_auto_swap``, wider ones by
+                    ``nonlocal_gates.mps_gate_nonlocal``
+      'nonlocal'    every gate on two or more sites by ``mps_gate_nonlocal``
+
+    Under 'auto-mps' and 'nonlocal' an entry may also be
+    ``(G, qubits, controls)``, applied by ``nonlocal_gates.mps_gate_controlled``,
+    and ``compress_opts`` (``max_bond``, ``cutoff`` ...) go to every gate;
+    ``method`` names the sub-MPO compression ('direct', 'dm', 'zipup') and
+    goes to the sub-MPO gates only.  One ``info`` dict (``compress_opts["info"]``, or a new one)
+    carries the orthogonality centre from gate to gate, so a gate whose span
+    already holds the centre skips canonicalisation."""
     compress_opts.setdefault("cutoff", 1e-10)
-    for G, where in gates:
-        where = tuple(where)
-        if len(where) == 1:
+    if contract not in ("swap+split", "auto-mps", "nonlocal"):
+        raise ValueError(f"apply_circuit: unknown contract mode {contract!r}")
+    if contract == "swap+split":
+        for entry in gates:
+            if len(entry) != 2:
+                raise ValueError("apply_circuit: controlled gates need contract='auto-mps' "
+                                 "or 'nonlocal'")
+            G, where = entry
+            where = tuple(where)
+            if len(where) == 1:
+                gate_single(sites, G, where[0])
+            elif len(where) == 2:
+                gate_with_auto_swap(sites, G, where, **compress_opts)
+            else:
+                raise ValueError("apply_circuit: only one- and two-qubit gates")
+        return sites
+    from . import nonlocal_gates as nl
+    info = compress_opts.pop("info", None)
+    if info is None:
+        info = {}
+    swap_opts = {k: v for k, v in compress_opts.items() if k != "method"}
+    for entry in gates:
+        G, where = entry[0], tuple(int(w) for w in entry[1])
+        controls = tuple(entry[2]) if len(entry) > 2 else ()
+        if controls:
+            sites[:] = nl.mps_gate_controlled(sites, G, where, controls, info=info,
+                                              **compress_opts)
+        elif len(where) == 1:
             gate_single(sites, G, where[0])
-        elif len(where) == 2:
-            gate_with_auto_swap(sites, G, where, **compress_opts)
+            # a non-unitary gate leaves its site no longer an isometry
+            cur = info.get("cur_orthog")
+            if isinstance(cur, tuple):
+                info["cur_orthog"] = (min(cur[0], where[0]), max(cur[1], where[0]))
+        elif len(where) == 2 and contract == "auto-mps":
+            gate_with_auto_swap(sites, G, where, **swap_opts)
+            # every site outside the gate's span is an isometry afterwards
+            info["cur_orthog"] = (min(where), max(where))
         else:
-            raise ValueError("apply_circuit: only one- and two-qubit gates")
+            sites[:] = nl.mps_gate_nonlocal(sites, G, where, info=info, **compress_opts)
     return sites
 
 
