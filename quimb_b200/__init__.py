@@ -26,7 +26,7 @@ from .tree import (ContractExpression, GraphedContraction, Tree,  # noqa: F401
                    gen_output_inds, tensor_contract)
 from .mps import (ChainPlan, MovingEnvironment, compute_left_environments,  # noqa: F401
                   compute_right_environments, env_left_step, env_right_step,
-                  mpo_ham_heis, mps_expec, mps_norm, mps_norm2)
+                  mpo_ham_heis, mps_expec, mps_expec2, mps_norm, mps_norm2)
 from .split import (array_split, array_svals, cholesky_regularized,  # noqa: F401
                     eigh_truncated, lddiv, ldmul, lu_truncated, polar_left, polar_right,
                     qr_stabilized, qr_via_cholesky, rddiv, rdmul, safe_inverse, sgn, svd_rand_truncated, svd_truncated,
@@ -40,6 +40,7 @@ from .tebd import (TEBD, LocalHam1D, gate_split, gate_with_auto_swap,  # noqa: F
 from .boundary import (BoundaryContractor2D, contract_boundary,  # noqa: F401
                        contract_boundary_two_sided, peps_norm_tensors)
 from .dmrg import DMRG1, DMRG2  # noqa: F401
+from .dmrgx import DMRGX  # noqa: F401
 from . import observables  # noqa: F401
 from .observables import (mps_calc_current_orthog_center, mps_canonicalize,  # noqa: F401
                           mps_compute_local_expectation, mps_correlation,

@@ -372,6 +372,10 @@ class DMRG2:
     def sweep_left(self, canonize=True, verbosity=0, **update_opts):
         return self.sweep("L", canonize=canonize, verbosity=verbosity, **update_opts)
 
+    def _compute_post_sweep(self):
+        """Per-sweep work after the energy is recorded (dmrg.py:1129); DMRG-X
+        records the variance here."""
+
     def _check_convergence(self, tol):
         if len(self.energies) < 2:
             return False
@@ -401,6 +405,7 @@ class DMRG2:
                                 cutoff_mode=self.opts["bond_compress_cutoff_mode"],
                                 method=self.opts["bond_compress_method"])
             self.energies.append(energy)
+            self._compute_post_sweep()
             if verbosity:
                 print(f"sweep {len(self.energies)} {direction} max_bond={max_bond} "
                       f"E={energy}", flush=True)

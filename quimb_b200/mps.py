@@ -63,12 +63,16 @@ def mpo_lrud(w, shape, i, n):
     return Array(t.permute(*(lay.index(c) for c in "lrud")), w.cj)
 
 
-def norm_step(E, A):
-    """E'[b', b] = sum_{a', a, p} E[a', a] conj(A)[a', p, b'] A[a, p, b]"""
+def norm_step(E, A, B=None):
+    """E'[b', b] = sum_{a', a, p} E[a', a] conj(B)[a', p, b'] A[a, p, b]
+
+    ``B`` (the bra site, default ``A``) may have other bonds than ``A``: the
+    overlap <phi|psi> of two states carries a (chi_phi, chi_psi) environment."""
+    B = A if B is None else B
     T = contract_pair(E.t, [LB_, L_], A.t, [L_, P_, R_], [LB_, P_, R_],
                       conj_a=E.cj, conj_b=A.cj)
-    return Array(contract_pair(A.t, [LB_, P_, RB_], T, [LB_, P_, R_],
-                               [RB_, R_], conj_a=not A.cj))
+    return Array(contract_pair(B.t, [LB_, P_, RB_], T, [LB_, P_, R_],
+                               [RB_, R_], conj_a=not B.cj))
 
 
 def _is_host(x):
@@ -235,6 +239,60 @@ def mps_expec(sites, mpo, shape="lrp", mpo_shape="lrud"):
     return E.reshape(())
 
 
+# labels of the second MPO layer of <psi|H.H|psi>: its bonds and the
+# physical index between the two layers
+W2_, WN2_, M_ = 8, 9, 10
+
+
+def env2_left_step(E, A, W):
+    """Two-layer step of <psi|H.H|psi>, ket-side layer first (the reference's
+    ``TN_energy2``, tn1d/dmrg.py:1219-1225):
+
+    E'[b', w1', w2', b] = sum E[a', w1, w2, a] A[a, p, b] W[w1, w1', p, m]
+                              W[w2, w2', m, q] conj(A)[a', q, b']
+
+    Four launches of the contraction kernel, 2 d w^2 chi^3 (x2) +
+    2 d^2 w^3 chi^2 (x2) flops."""
+    T = contract_pair(E.t, [LB_, W_, W2_, L_], A.t, [L_, P_, R_],
+                      [LB_, W_, W2_, P_, R_], conj_a=E.cj, conj_b=A.cj)
+    T = contract_pair(T, [LB_, W_, W2_, P_, R_], W.t, [W_, WN_, P_, M_],
+                      [LB_, M_, WN_, W2_, R_], conj_b=W.cj)
+    T = contract_pair(T, [LB_, M_, WN_, W2_, R_], W.t, [W2_, WN2_, M_, PB_],
+                      [LB_, PB_, WN_, WN2_, R_], conj_b=W.cj)
+    return Array(contract_pair(A.t, [LB_, PB_, RB_], T, [LB_, PB_, WN_, WN2_, R_],
+                               [RB_, WN_, WN2_, R_], conj_a=not A.cj))
+
+
+def env2_right_step(E, A, W):
+    """E'[a', w1, w2, a] = sum A[a, p, b] E[b', w1', w2', b] W[w1, w1', p, m]
+    W[w2, w2', m, q] conj(A)[a', q, b']  (mirror of :func:`env2_left_step`)"""
+    T = contract_pair(A.t, [L_, P_, R_], E.t, [RB_, WN_, WN2_, R_],
+                      [L_, P_, WN_, WN2_, RB_], conj_a=A.cj, conj_b=E.cj)
+    T = contract_pair(W.t, [W_, WN_, P_, M_], T, [L_, P_, WN_, WN2_, RB_],
+                      [W_, L_, M_, WN2_, RB_], conj_a=W.cj)
+    T = contract_pair(W.t, [W2_, WN2_, M_, PB_], T, [W_, L_, M_, WN2_, RB_],
+                      [W_, W2_, L_, PB_, RB_], conj_a=W.cj)
+    return Array(contract_pair(A.t, [LB_, PB_, RB_], T, [W_, W2_, L_, PB_, RB_],
+                               [LB_, W_, W2_, L_], conj_a=not A.cj))
+
+
+def mps_expec2(sites, mpo, shape="lrp", mpo_shape="lrud"):
+    """<psi|H.H|psi> (the reference's ``TN_energy2 ^ ...``,
+    tn1d/dmrg.py:1219-1227): with :func:`mps_expec`, the energy variance
+    <H^2> - <H>^2 that certifies an eigenstate; 0-d Array."""
+    n = len(sites)
+    E = None
+    for i in range(n):
+        A = site_lpr(sites[i], shape, i, n)
+        W = mpo_lrud(mpo[i], mpo_shape, i, n)
+        if W.dtype != A.dtype:
+            W = W.astype(A.dtype)
+        if E is None:
+            E = ops.ones((1, 1, 1, 1), dtype=A.dtype, device=A.device)
+        E = env2_left_step(E, A, W)
+    return E.reshape(())
+
+
 # ------------------------------------------------------------ environments ---
 def compute_left_environments(sites, mpo=None, shape="lrp", mpo_shape="lrud"):
     """Left environments of <psi|psi> (``mpo=None``: (chi, chi) arrays) or
@@ -260,12 +318,14 @@ def compute_left_environments(sites, mpo=None, shape="lrp", mpo_shape="lrud"):
     return envs
 
 
-def norm_step_right(E, A):
-    """E'[a', a] = sum_{b', b, p} conj(A)[a', p, b'] A[a, p, b] E[b', b]"""
+def norm_step_right(E, A, B=None):
+    """E'[a', a] = sum_{b', b, p} conj(B)[a', p, b'] A[a, p, b] E[b', b]
+    (``B``: the bra site, default ``A``)"""
+    B = A if B is None else B
     T = contract_pair(A.t, [L_, P_, R_], E.t, [RB_, R_], [L_, P_, RB_],
                       conj_a=A.cj, conj_b=E.cj)
-    return Array(contract_pair(A.t, [LB_, P_, RB_], T, [L_, P_, RB_],
-                               [LB_, L_], conj_a=not A.cj))
+    return Array(contract_pair(B.t, [LB_, P_, RB_], T, [L_, P_, RB_],
+                               [LB_, L_], conj_a=not B.cj))
 
 
 def compute_right_environments(sites, mpo=None, shape="lrp", mpo_shape="lrud"):
