@@ -201,6 +201,19 @@ int qb_contract_pair_feed(const qb_tensor_t *A, const int32_t *labelsA,
                           int64_t *out2);
 
 /*
+ * Host-only: how the stream-K grid of qb_contract_pair_route (engine = auto)
+ * splits its work.  out[0] = 1 pair schedule (2-CTA clusters, one per tile,
+ * each CTA one k-half, summed in distributed shared memory), 0 the segment
+ * loop (equal-cost k-block ranges, partial tiles summed through the
+ * workspace), -1 the route is not stream-K.  Without a device it assumes
+ * that half the planner's grid can run as clusters at once.
+ */
+int qb_contract_pair_schedule(const qb_tensor_t *A, const int32_t *labelsA,
+                              const qb_tensor_t *B, const int32_t *labelsB,
+                              const qb_tensor_t *C, const int32_t *labelsC,
+                              int64_t *out1);
+
+/*
  * TEST / debug entry, host pointers only: runs the streaming engine's row
  * code (shared __host__ __device__ functions of contract_stream.cu) in a
  * host loop so that its index bookkeeping can be checked without a device.

@@ -19,7 +19,8 @@ from .array import Array
 from .ops import *  # noqa: F401,F403  (the autoray-visible function surface)
 from .ops import (abs, all, any, max, min, sum)  # noqa: F401,A004
 from . import linalg  # noqa: F401
-from .contract import contract_batched, contract_pair, feed_pair, plan_pair, route_pair  # noqa: F401
+from .contract import (contract_batched, contract_pair, feed_pair, plan_pair,  # noqa: F401
+                       route_pair, schedule_pair)
 from . import dist  # noqa: F401
 from .tree import (ContractExpression, GraphedContraction, Tree,  # noqa: F401
                    array_contract, find_sliced_tree, find_slices, find_tree,

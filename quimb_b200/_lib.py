@@ -88,6 +88,7 @@ def load(build_if_missing=True):
     sig("qb_contract_pair_plan", ci, [T, I32P, T, I32P, T, I32P, P(i64)])
     sig("qb_contract_pair_route", ci, [T, I32P, T, I32P, T, I32P, ci, P(i64)])
     sig("qb_contract_pair_feed", ci, [T, I32P, T, I32P, T, I32P, P(i64)])
+    sig("qb_contract_pair_schedule", ci, [T, I32P, T, I32P, T, I32P, P(i64)])
     sig("qb_contract_batched", ci,
         [T, I32P, T, I32P, T, I32P, vp, vp, vp, i64, ci, ci, vp])
     sig("qb_permute", ci, [T, T, ci, vp])

@@ -362,6 +362,29 @@ def feed_pair(a_shape, a_strides, la, b_shape, b_strides, lb, c_shape,
     return {"A": FEEDS[out[0]], "B": FEEDS[out[1]]}
 
 
+SCHEDULES = {1: "pair", 0: "segments", -1: None}
+
+
+def schedule_pair(a_shape, a_strides, la, b_shape, b_strides, lb, c_shape,
+                  c_strides, lc, dtype_code=_lib.QB_F64, ptrs=None):
+    """Host-only: how the stream-K grid of ``route_pair`` (engine auto) runs:
+    ``"pair"`` (2-CTA clusters, one per tile, each CTA one k-half, the halves
+    summed in distributed shared memory), ``"segments"`` (equal-cost k-block
+    ranges, partial tiles summed through the workspace) or None when the
+    route is not stream-K.  Without a device, half the grid is assumed to fit
+    as clusters at once.  ``ptrs`` as for ``route_pair``."""
+    lib = _lib.load()
+    pa, pb, pc = ptrs if ptrs is not None else (0x10000000,) * 3
+    da = _lib.np_desc(a_shape, a_strides, dtype_code, pa)
+    db = _lib.np_desc(b_shape, b_strides, dtype_code, pb)
+    dc = _lib.np_desc(c_shape, c_strides, dtype_code, pc)
+    out = (ctypes.c_int64 * 1)()
+    rc = lib.qb_contract_pair_schedule(da, _lib.labels(la), db, _lib.labels(lb),
+                                       dc, _lib.labels(lc), out)
+    _lib.check(rc, "qb_contract_pair_schedule")
+    return SCHEDULES[out[0]]
+
+
 def contract_batched(a_list, la, b_list, lb, lc, conj_a=False, conj_b=False):
     """Many independent contractions of identical signature in ONE launch
     (the small same-shape intermediates of MPS / PEPS / circuit sweeps).

@@ -197,6 +197,17 @@ int qb_contract_pair_feed(const qb_tensor_t *A, const int32_t *la,
   return 0;
 }
 
+int qb_contract_pair_schedule(const qb_tensor_t *A, const int32_t *la,
+                              const qb_tensor_t *B, const int32_t *lb,
+                              const qb_tensor_t *C, const int32_t *lc, int64_t *out) {
+  PairPlan plan;
+  int rc = plan_pair(A, la, B, lb, C, lc, 0, 0, plan);
+  if (rc) return rc;
+  const Route r = select_route(plan, QB_ENGINE_AUTO);
+  out[0] = r.kind != ROUTE_DMMA_STREAMK ? -1 : (streamk_pair(plan) ? 1 : 0);
+  return 0;
+}
+
 int64_t qb_contract_pair_workspace(const qb_tensor_t *A, const int32_t *la,
                                    const qb_tensor_t *B, const int32_t *lb,
                                    const qb_tensor_t *C, const int32_t *lc,

@@ -208,6 +208,29 @@ __device__ __forceinline__ unsigned long long global_ns() {
       p.trace[((size_t)sk.bid * 4 + sk.seg) * 8 + (ph)] = global_ns();      \
   } while (0)
 
+// thread-block cluster primitives (the stream-K pair schedule)
+__device__ __forceinline__ int cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return (int)r;
+}
+// every thread of both CTAs arrives; writes before it are visible after it
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\t"
+               "barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the address of the same shared-memory byte in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t cluster_map(uint32_t addr, int rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+  return r;
+}
+__device__ __forceinline__ double ld_cluster(uint32_t addr) {
+  double v;
+  asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(addr));
+  return v;
+}
+
 // stream-K bookkeeping of one tile segment
 struct SkSeg {
   int mode;        // 0: classic tile, 1: tail (write partial), 2: head (sum peers)
@@ -219,9 +242,12 @@ struct SkSeg {
 };
 
 // FEED: bit 0 / bit 1 = A / B gathered by the affine feed (real operands with
-// a compile-time layout only); 0 = offset tables for both
+// a compile-time layout only); 0 = offset tables for both.
+// PAIR: [kbeg, kend) is one k-half of the tile and the other CTA of this
+// 2-CTA cluster runs the other half (streamk_pair_grid); the two halves are
+// summed through distributed shared memory and each CTA stores half the rows
 template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
-          bool CPLX, int LA = -1, int LB = -1, int FEED = 0>
+          bool CPLX, int LA = -1, int LB = -1, int FEED = 0, bool PAIR = false>
 __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
                                               int64_t zb, int ks, int64_t kbeg,
                                               int64_t kend, const SkSeg sk) {
@@ -515,9 +541,45 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
     }
   }
 
+  // ---- stream-K pair: rank r stores warp row r of the tile; the other warp
+  // row parks its accumulators in this CTA's (now idle) ring for the peer ----
+  bool own = true;
+  if constexpr (PAIR) {
+    constexpr int HALF = NT / WARPS_M;  // threads of one warp row
+    static_assert(WARPS_M == 2, "one warp row per CTA of the pair");
+    static_assert((size_t)MT * NT8 * 4 * HALF <= (size_t)STAGES * Cfg::A_ELEMS,
+                  "parked half fits the A ring");
+    const int rank = cluster_ctarank();
+    own = warp / WARPS_N == rank;
+    const int slot = tid % HALF;
+    __syncthreads();  // no warp reads the ring any more
+    if (!own) {
+#pragma unroll
+      for (int i = 0; i < MT; ++i)
+#pragma unroll
+        for (int j = 0; j < NT8; ++j)
+#pragma unroll
+          for (int v = 0; v < 4; ++v) sA[((i * NT8 + j) * 4 + v) * HALF + slot] = acc[i][j][v];
+    }
+    cluster_sync();  // both parked halves visible cluster-wide
+    if (own) {
+      // the peer's warps of this warp row ran the other k-half of these rows;
+      // a + b == b + a, so both CTAs' sums are the same whichever half is local
+      const uint32_t peer = cluster_map(smem_u32(sA + slot), rank ^ 1);
+#pragma unroll
+      for (int i = 0; i < MT; ++i)
+#pragma unroll
+        for (int j = 0; j < NT8; ++j)
+#pragma unroll
+          for (int v = 0; v < 4; ++v)
+            acc[i][j][v] += ld_cluster(peer + ((i * NT8 + j) * 4 + v) * HALF * 8);
+    }
+    cluster_sync();  // the peer has read this CTA's shared memory: it may exit
+  }
+
   QB_TRACE(5);
   // ---- epilogue ----------------------------------------------------------
-  if (p.splitk > 1) {
+  if (!PAIR && p.splitk > 1) {
     // canonical [split][batch][M][Nh] partial buffer
     double *P = p.partial + ((int64_t)ks * p.nbatch + zb) * p.M * Nh;
 #pragma unroll
@@ -542,7 +604,7 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = wm0 + i * 16 + g + h * 8;
-      const int64_t om = offCm[r];
+      const int64_t om = own ? offCm[r] : -1;
       if (om < 0) continue;
 #pragma unroll
       for (int j = 0; j < NT8; ++j) {
@@ -571,6 +633,10 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
         }
       }
     }
+  // pair: thread 0 of rank 1 stores nothing; stamp once the owners have
+  if constexpr (PAIR) {
+    if (p.trace) __syncthreads();
+  }
   QB_TRACE(6);
 }
 
@@ -660,6 +726,40 @@ __global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
   streamk_grid<BM, BN, BK, WARPS_M, WARPS_N, STAGES, false, LA, LB, FEED>(p);
 }
 
+// Stream-K pair schedule, for a stream-K grid with at most half as many tiles
+// as CTAs: the equal-cost cut is then "every tile in two halves".  The grid
+// runs as clusters of 2 CTAs; cluster c takes tile c (the same grouped
+// rasterisation), rank 0 its first nkbT/2 k-blocks and rank 1 the rest, and
+// the two halves are summed in distributed shared memory (contract_tile,
+// PAIR): no workspace, no flags, and no wait outside the cluster.
+template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
+          bool CPLX, int LA, int LB, int FEED>
+__device__ __forceinline__ void streamk_pair_grid(const ContractParams &p) {
+  const int tile = blockIdx.x / 2;
+  // surplus clusters: both CTAs leave here, before either reaches a barrier
+  if (tile >= p.tiles_m * p.tiles_n) return;
+  const int64_t Kh = CPLX ? 2 * p.K : p.K;
+  const int64_t kmid = (Kh + BK - 1) / BK / 2 * BK;
+  const int rank = cluster_ctarank();
+  SkSeg sk{0, (int)blockIdx.x, 0, 0, nullptr, nullptr, 0};
+  contract_tile<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB, FEED, true>(
+      p, tile, 0, 0, rank ? kmid : 0, rank ? Kh : kmid, sk);
+}
+
+template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES,
+          bool CPLX, int LA = -1, int LB = -1>
+__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
+    contract_f64_pair_kernel(const __grid_constant__ ContractParams p) {
+  streamk_pair_grid<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB, 0>(p);
+}
+
+template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES, int LA,
+          int LB, int FEED>
+__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
+    contract_f64_affine_pair_kernel(const __grid_constant__ ContractParams p) {
+  streamk_pair_grid<BM, BN, BK, WARPS_M, WARPS_N, STAGES, false, LA, LB, FEED>(p);
+}
+
 // deterministic split-K reduction + strided scatter into C
 template <bool CPLX>
 __global__ void splitk_reduce_f64_kernel(const __grid_constant__ ContractParams p) {
@@ -700,22 +800,32 @@ __global__ void splitk_reduce_f64_kernel(const __grid_constant__ ContractParams 
 // their offset tables, then block in griddepcontrol.wait until it has
 // completed and flushed), which hides the launch latency between the
 // back-to-back contractions of a tree / an MPS sweep.  Launches recorded into
-// a stream capture go without the attribute.
+// a stream capture go without the attribute.  cluster > 1: CTAs are launched
+// in thread-block clusters of that many along x.
 template <typename Kern>
 static int launch_pdl(Kern kern, dim3 grid, int threads, size_t smem, cudaStream_t st,
-                      const ContractParams &p) {
+                      const ContractParams &p, int cluster = 1) {
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute attr[1];
+  cudaLaunchAttribute attr[2];
+  unsigned n = 0;
+  if (cluster > 1) {
+    attr[n].id = cudaLaunchAttributeClusterDimension;
+    attr[n].val.clusterDim.x = cluster;
+    attr[n].val.clusterDim.y = 1;
+    attr[n].val.clusterDim.z = 1;
+    ++n;
+  }
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   cudaStreamIsCapturing(st, &cap);
   if (cap == cudaStreamCaptureStatusNone) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n].val.programmaticStreamSerializationAllowed = 1;
+    ++n;
   }
+  cfg.attrs = n ? attr : nullptr; cfg.numAttrs = n;
   QB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, p));
   QB_LAUNCH_CHECK();
   return 0;
@@ -752,9 +862,74 @@ static int launch_cfg(const ContractParams &p, cudaStream_t st) {
 // (a_kmajor / b_kmajor, plan.h), which the route carries, and on which
 // operands the planner proved affine (feedA / feedB).  The complex kernel
 // takes its layout at run time and always gathers through the tables.
+using LargeCfg = KernelCfg<128, 128, 32, 2, 4, 3>;
+
+// 2-CTA clusters of the large tile that the current device holds at once,
+// asked once per device; -1 without a device.  Every pair kernel has the same
+// block, the same shared memory and one CTA per SM, so one kernel answers for
+// all of them.
+static int pair_active_clusters() {
+  constexpr int kMaxDevices = 64;
+  static std::atomic<int> known[kMaxDevices];  // clusters + 1; 0 = not asked yet
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev >= kMaxDevices) {
+    cudaGetLastError();
+    return -1;
+  }
+  int n = known[dev].load();
+  if (n) return n - 1;
+  auto kern = contract_f64_pair_kernel<128, 128, 32, 2, 4, 3, true>;
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(2); cfg.blockDim = dim3(LargeCfg::NT);
+  cfg.dynamicSmemBytes = LargeCfg::SMEM;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+  cfg.attrs = &attr; cfg.numAttrs = 1;
+  n = 0;
+  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)LargeCfg::SMEM) != cudaSuccess ||
+      cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) {
+    cudaGetLastError();  // no pair schedule on this device
+    n = 0;
+  }
+  known[dev].store(n + 1);
+  return n;
+}
+
+bool streamk_pair(const PairPlan &plan) {
+  const int G = plan.streamk;
+  const int64_t tiles = (int64_t)plan.p.tiles_m * plan.p.tiles_n;
+  if (G <= 0 || G % 2 != 0 || tiles * 2 > G || plan.p.nbatch != 1) return false;
+  int clusters = pair_active_clusters();
+  if (clusters < 0) clusters = G / 2;
+  // all tiles in one wave of clusters
+  return clusters >= tiles;
+}
+
+// G CTAs as G/2 clusters; the flag words stay untouched (and zero)
+template <bool CPLX, int LA, int LB, int FEED>
+static int launch_pair_l(const PairPlan &plan, cudaStream_t st) {
+  auto kern = [] {
+    if constexpr (FEED == 0)
+      return contract_f64_pair_kernel<128, 128, 32, 2, 4, 3, CPLX, LA, LB>;
+    else
+      return contract_f64_affine_pair_kernel<128, 128, 32, 2, 4, 3, LA, LB, FEED>;
+  }();
+  static bool attr_set = false;
+  if (!attr_set) {
+    QB_CUDA_CHECK(cudaFuncSetAttribute(
+        kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LargeCfg::SMEM));
+    attr_set = true;
+  }
+  return launch_pdl(kern, dim3(plan.streamk), LargeCfg::NT, LargeCfg::SMEM, st, plan.p, 2);
+}
+
 template <bool CPLX, int LA, int LB, int FEED>
 static int launch_streamk_l(const PairPlan &plan, cudaStream_t st) {
-  using Cfg = KernelCfg<128, 128, 32, 2, 4, 3>;
+  if (streamk_pair(plan)) return launch_pair_l<CPLX, LA, LB, FEED>(plan, st);
+  using Cfg = LargeCfg;
   auto kern = [] {
     if constexpr (FEED == 0)
       return contract_f64_streamk_kernel<128, 128, 32, 2, 4, 3, CPLX, LA, LB>;

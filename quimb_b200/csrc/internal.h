@@ -10,6 +10,9 @@ namespace qb {
 
 int launch_contract_f64(const PairPlan &plan, cudaStream_t st);
 int launch_contract_c128(const PairPlan &plan, cudaStream_t st);
+// a stream-K route runs the pair schedule (2-CTA clusters, one per tile) rather
+// than the segment loop; qb_contract_pair_schedule reports it
+bool streamk_pair(const PairPlan &plan);
 int launch_fill_zero(const qb_tensor_t *C, cudaStream_t st);
 
 // int8 tensor-core (wgmma) error-free-split engine (ozaki_tc.cu)

@@ -8,7 +8,8 @@ its route (the stream-K grid is one CTA per SM).
   python tools/trace_contract.py [--out trace.json]
 
 phases: 0 entry, 1 tables done, 2 prologue issued, 3 first tile landed,
-        4 main loop done, 5 stream-K fix-up done, 6 stores issued
+        4 main loop done, 5 stream-K fix-up done (pair schedule: the
+        distributed-shared-memory exchange of the two k-halves), 6 stores issued
 """
 import ctypes
 import json
@@ -33,7 +34,7 @@ def read_trace():
     return np.frombuffer(buf, dtype=np.uint64).reshape(16, 8192).copy()
 
 
-def analyse(slot, G):
+def analyse(slot, G, schedule=None):
     t = slot[: G * 32].reshape(G, 4, 8).astype(np.int64)
     out = {}
     seg_used = (t[:, :, 0] > 0)
@@ -42,7 +43,8 @@ def analyse(slot, G):
     ends = np.where(seg_used, t[:, :, 6], 0).max(axis=1)
     out["start_ns"] = int(t0.min()); out["end_ns"] = int(ends.max())
     out["total_us"] = (out["end_ns"] - out["start_ns"]) / 1e3
-    names = ["tables", "prologue_issue", "first_tile_wait", "main_loop", "fixup", "stores"]
+    names = ["tables", "prologue_issue", "first_tile_wait", "main_loop",
+             "exchange" if schedule == "pair" else "fixup", "stores"]
     for s in range(4):
         m = seg_used[:, s]
         if not m.any():
@@ -90,6 +92,7 @@ def main():
         ptrs = (x.data_ptr(), y.data_ptr(), z.data_ptr())
         r = qb.route_pair(*args, ptrs=ptrs)
         f = qb.feed_pair(*args, ptrs=ptrs)
+        r["schedule"] = qb.schedule_pair(*args, ptrs=ptrs)
         tiles = (x.shape[0] // 128) * (z.numel() // x.shape[0] // 128) if r["streamk"] == 0 else 0
         grids.append((r["streamk"] or tiles, r, f))
         print(json.dumps({"route": r, "feed": f}))
@@ -97,7 +100,7 @@ def main():
     for n, i in enumerate(used):
         G, r, f = grids[n % 2]
         res.append({"kind": r["kind"], "layout": r["layout"], "ctas": G, "feed": f,
-                    **analyse(tr[i], G)})
+                    "schedule": r["schedule"], **analyse(tr[i], G, r["schedule"])})
     res.sort(key=lambda r: r["start_ns"])
     for k, r in enumerate(res):
         gap = (r["start_ns"] - res[k - 1]["end_ns"]) / 1e3 if k else None
