@@ -29,6 +29,9 @@
  *   qb_rdm_reduce         <- the final contraction of
  *                            MatrixProductState.partial_trace_to_dense_canonical
  *                            and of the local expectations, core.py:2827-3087
+ *   qb_plaquette_expec    <- the per-term contractions of
+ *                            PEPS.compute_local_expectation,
+ *                            quimb/tensor/tn2d/core.py:4335-4348
  *   qb_sketch_env         <- the noise-sketched left environments of
  *                            tensor_network_1d_compress_src,
  *                            quimb/tensor/tn1d/compress.py:1787-1826
@@ -413,6 +416,41 @@ int qb_rdm_reduce(int dtype, int64_t n1, int64_t M, int64_t N, int64_t n2,
                   const void *U, const int64_t ustride[3],
                   const void *V, const int64_t vstride[3],
                   void *out, void *workspace, int64_t ws_bytes, void *stream);
+
+/* ---- PEPS local expectations from plaquette density matrices ----------- */
+/*
+ * The per-term evaluation of PEPS.compute_local_expectation
+ * (quimb/tensor/tn2d/core.py:4335-4348), for every term of a call in one
+ * launch.  Term t reads row t of the host table `desc` (QB_PLAQ_DESC_WORDS
+ * int64 words):
+ *   [0] offset of its plaquette's rho (elements) in `rho`, a row-major D x D
+ *       matrix, ket index first; D = prod of the site dimensions <= 64
+ *   [1] offset of its G (elements) in `G`, a row-major dg x dg matrix over
+ *       the term's sites in increasing position order (out index first)
+ *   [2] number of plaquette sites, 1 .. QB_PLAQ_MAX_SITES
+ *   [3] number of term sites, 1 or 2
+ *   [4], [5] the term's site positions within the plaquette, increasing
+ *       ([5] unused for one site)
+ *   [6 .. 11] the plaquette's per-site dimensions
+ * and writes out[2 t] = Tr[G_t rho_p] with the other plaquette sites traced,
+ * out[2 t + 1] = Tr[rho_p].  rho, G and out are device arrays of one dtype,
+ * QB_F64 or QB_C128.  The table is copied once to the device buffer
+ * `desc_dev` (n_terms * QB_PLAQ_DESC_WORDS int64) on `stream`, then one
+ * kernel runs there; no allocation, no host synchronisation.  Pageable `desc`
+ * may be reused when the call returns.  Every sum has a fixed order set by
+ * the descriptor alone: the same input gives the same bits on any device or
+ * stream, and NaN / Inf reach only the terms that read them.
+ * Unknown dtype (-1), n_terms < 0 (-2), an invalid descriptor: counts,
+ * positions, dimensions, D > 64 or an offset out of rho_elems / g_elems (-3),
+ * a pointer null or misaligned (-4); nothing is copied or launched when a
+ * call is rejected, and n_terms == 0 does nothing.
+ */
+#define QB_PLAQ_DESC_WORDS 12
+#define QB_PLAQ_MAX_SITES 6
+#define QB_PLAQ_MAX_DIM 64
+int qb_plaquette_expec(int dtype, int64_t n_terms, const int64_t *desc, void *desc_dev,
+                       const void *rho, int64_t rho_elems, const void *G, int64_t g_elems,
+                       void *out, void *stream);
 
 /* ---- sketched left environments of successive randomized compression --- */
 /*

@@ -42,6 +42,9 @@ from .boundary import (BoundaryContractor2D, contract_boundary,  # noqa: F401
                        contract_boundary_two_sided, peps_norm_tensors)
 from .dmrg import DMRG1, DMRG2  # noqa: F401
 from .dmrgx import DMRGX  # noqa: F401
+from . import peps_expec  # noqa: F401
+from .peps_expec import (calc_plaquette_map, calc_plaquette_sizes,  # noqa: F401
+                         peps_compute_local_expectation, peps_normalize, plaquette_to_sites)
 from . import observables  # noqa: F401
 from .observables import (mps_calc_current_orthog_center, mps_canonicalize,  # noqa: F401
                           mps_compute_local_expectation, mps_correlation,

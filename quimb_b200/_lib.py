@@ -14,6 +14,7 @@ QB_MAX_RANK = 32
 QB_F32, QB_F64, QB_C64, QB_C128 = 0, 1, 2, 3
 QB_ENGINE_AUTO, QB_ENGINE_DMMA, QB_ENGINE_OZAKI, QB_ENGINE_STREAM = 0, 1, 2, 3
 QB_ENGINE_WS_ZEROED = 0x100
+QB_PLAQ_DESC_WORDS = 12
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libquimb_b200.so")
@@ -107,6 +108,7 @@ def load(build_if_missing=True):
     sig("qb_sample_select", ci, [ci, i64, i64, i64, vp, vp, i64, vp, i64, vp, vp, vp])
     sig("qb_rdm_workspace", i64, [i64, i64, i64, i64])
     sig("qb_rdm_reduce", ci, [ci, i64, i64, i64, i64, vp, P(i64), vp, P(i64), vp, vp, i64, vp])
+    sig("qb_plaquette_expec", ci, [ci, i64, P(i64), vp, vp, i64, vp, i64, vp, vp])
     sig("qb_sketch_env", ci, [ci, i64, i64, i64, i64, i64, i64, vp, P(i64), vp, P(i64), vp,
                               P(i64), vp, P(i64), vp])
     for name, res, args in (

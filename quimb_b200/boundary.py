@@ -320,6 +320,167 @@ class BoundaryContractor2D:
         return data if inds else (data.item() if isinstance(data, Array) else data)
 
 
+    # ---- environments (tn2d/core.py:2716-2835, :3075-3431) ------------------
+    # An environment is a snapshot ``{(i, j): [LTensor, ...]}`` of the tensors
+    # the reference selects by tag: the boundary line (or the raw first line,
+    # or one dense tensor) on the coordinates it was contracted onto.  The
+    # snapshot holds its own LTensor wrappers: canonize / compress replace
+    # ``.data`` of the wrappers they touch with new arrays and never write into
+    # an array, so a snapshot shares device memory but no mutable state.
+    def _copy(self):
+        bc = BoundaryContractor2D.__new__(BoundaryContractor2D)
+        bc.Lx, bc.Ly = self.Lx, self.Ly
+        bc.sites = {c: [_clone(t) for t in ts] for c, ts in self.sites.items()}
+        bc.n_compress, bc.max_bond_seen = 0, 1
+        return bc
+
+    def _snapshot(self, coos):
+        return {c: [_clone(t) for t in self.sites[c]] for c in coos if self.sites[c]}
+
+    def compute_environments(self, from_which, xrange=None, yrange=None, max_bond=None, *,
+                             cutoff=1e-10, canonize=True, layer_tags=None, dense=False):
+        """``envs[from_which, i]`` for every line ``i`` of the sweep
+        (compute_environments, tn2d/core.py:2716-2835): empty for the first
+        line, the raw first line for the second, then the boundary after each
+        inward step, or with ``dense`` the exact contraction of every line so
+        far into one tensor.  The contractor itself is left unchanged."""
+        if from_which not in ("xmin", "xmax", "ymin", "ymax"):
+            raise ValueError(f"invalid boundary direction {from_which!r}")
+        xrange = (0, self.Lx - 1) if xrange is None else tuple(xrange)
+        yrange = (0, self.Ly - 1) if yrange is None else tuple(yrange)
+        tn = self._copy()
+        plane = from_which[0]
+        irange, jrange = (xrange, yrange) if plane == "x" else (yrange, xrange)
+        imin, imax = sorted(irange)
+        step = +1 if "min" in from_which else -1
+        sweep = list(range(imin, imax + 1)) if step > 0 else list(range(imax, imin - 1, -1))
+        n_other = self.Ly if plane == "x" else self.Lx
+        jmin = min(jrange)
+
+        def site(i, j):
+            return (i, j) if plane == "x" else (j, i)
+
+        def line(i):
+            # a line tag selects the whole row / column, not just jrange
+            return [site(i, j) for j in range(n_other)]
+
+        def merge_lines(*lines):
+            ts = [t for i in lines for c in line(i) for t in tn.sites[c]]
+            for i in lines:
+                for c in line(i):
+                    tn.sites[c] = []
+            tn.sites[site(lines[-1], jmin)] = [_contract(ts)]
+
+        envs = {(from_which, sweep[0]): {}}
+        if len(sweep) < 2:
+            return envs
+        if dense:
+            merge_lines(sweep[0])
+        envs[from_which, sweep[1]] = tn._snapshot(line(sweep[0]))
+        for i in sweep[2:]:
+            iprevprev, iprev = i - 2 * step, i - step
+            if dense:
+                merge_lines(iprevprev, iprev)
+            else:
+                xr = (iprevprev, iprev) if plane == "x" else xrange
+                yr = (iprevprev, iprev) if plane == "y" else yrange
+                tn.contract_boundary_from(xr, yr, from_which, max_bond, cutoff=cutoff,
+                                          canonize=canonize, layer_tags=layer_tags)
+            envs[from_which, i] = tn._snapshot(line(iprev))
+        return envs
+
+    def compute_x_environments(self, max_bond=None, *, cutoff=1e-10, canonize=True,
+                               layer_tags=None, dense=False, yrange=None):
+        """The 'xmin' and 'xmax' environments of every row."""
+        envs = {}
+        for side in ("xmin", "xmax"):
+            envs.update(self.compute_environments(side, None, yrange, max_bond, cutoff=cutoff,
+                                                  canonize=canonize, layer_tags=layer_tags,
+                                                  dense=dense))
+        return envs
+
+    def compute_y_environments(self, max_bond=None, *, cutoff=1e-10, canonize=True,
+                               layer_tags=None, dense=False, xrange=None):
+        """The 'ymin' and 'ymax' environments of every column."""
+        envs = {}
+        for side in ("ymin", "ymax"):
+            envs.update(self.compute_environments(side, xrange, None, max_bond, cutoff=cutoff,
+                                                  canonize=canonize, layer_tags=layer_tags,
+                                                  dense=dense))
+        return envs
+
+    def compute_plaquette_environments(self, x_bsz=2, y_bsz=2, max_bond=None, *,
+                                       cutoff=1e-10, canonize=True, layer_tags=None,
+                                       first_contract=None, second_dense=None):
+        """``{((i0, j0), (x_bsz, y_bsz)): [LTensor, ...]}``: the environment of
+        every plaquette of the given size (compute_plaquette_environments,
+        tn2d/core.py:3324-3431).  Rows (``first_contract='x'``) or columns
+        are contracted from both sides first; then each strip of ``x_bsz``
+        rows (``y_bsz`` columns) between its two environments is contracted
+        from both ends in the rotated direction, exactly (``second_dense``,
+        the default for a block size of 1) or by boundary sweeps."""
+        if first_contract is None:
+            if x_bsz != y_bsz:
+                first_contract = "y" if x_bsz > y_bsz else "x"
+            else:
+                first_contract = "x" if self.Lx >= self.Ly else "y"
+        if first_contract not in ("x", "y"):
+            raise ValueError(f"first_contract must be 'x' or 'y', got {first_contract!r}")
+        opts = dict(max_bond=max_bond, cutoff=cutoff, canonize=canonize, layer_tags=layer_tags)
+        x_first = first_contract == "x"
+        # the first direction's block size, lattice length and coordinate order
+        bsz, osz = (x_bsz, y_bsz) if x_first else (y_bsz, x_bsz)
+        L = self.Lx if x_first else self.Ly
+        if second_dense is None:
+            second_dense = bsz < 2
+        first = (self.compute_x_environments if x_first else self.compute_y_environments)(**opts)
+        a, b = ("xmin", "xmax") if x_first else ("ymin", "ymax")
+        c, d = ("ymin", "ymax") if x_first else ("xmin", "xmax")
+
+        def coo(i, j):   # (first-direction index, other index) -> site
+            return (i, j) if x_first else (j, i)
+
+        strips = {}
+        for i in range(L - bsz + 1):
+            strip = BoundaryContractor2D.__new__(BoundaryContractor2D)
+            strip.Lx, strip.Ly = self.Lx, self.Ly
+            strip.sites = {cc: [] for cc in self.sites}
+            strip.n_compress, strip.max_bond_seen = 0, 1
+            for env in (first[a, i], first[b, i + bsz - 1]):
+                for cc, ts in env.items():
+                    strip.sites[cc] += [_clone(t) for t in ts]
+            for cc, ts in self.sites.items():
+                if i <= cc[0 if x_first else 1] < i + bsz:
+                    strip.sites[cc] += [_clone(t) for t in ts]
+            rng = (max(i - 1, 0), min(i + bsz, L - 1))
+            second = strip.compute_y_environments if x_first else strip.compute_x_environments
+            strips[i] = second(dense=second_dense, **opts,
+                               **({"xrange": rng} if x_first else {"yrange": rng}))
+
+        def select(env, coos):
+            return [t for cc in coos if cc in env for t in env[cc]]
+
+        out = {}
+        for i0, j0 in itertools.product(range(L - bsz + 1),
+                                        range((self.Ly if x_first else self.Lx) - osz + 1)):
+            # the rotated strip's ends span the first-direction neighbours too
+            side_lo = [coo(i0 + x, j0 - 1) for x in range(-1, bsz + 1)]
+            side_hi = [coo(i0 + x, j0 + osz) for x in range(-1, bsz + 1)]
+            below = [coo(i0 - 1, j0 + y) for y in range(osz)]
+            above = [coo(i0 + bsz, j0 + y) for y in range(osz)]
+            env = (select(strips[i0][c, j0], side_lo) + select(strips[i0][d, j0 + osz - 1], side_hi)
+                   + select(first[a, i0], below) + select(first[b, i0 + bsz - 1], above))
+            (p0, p1), size = coo(i0, j0), (x_bsz, y_bsz)
+            out[(p0, p1), size] = env
+        return out
+
+
+def _clone(t):
+    c = LTensor.__new__(LTensor)
+    c.data, c.inds, c.layer, c.left_inds = t.data, t.inds, t.layer, t.left_inds
+    return c
+
+
 def contract_boundary(tensors, Lx, Ly, max_bond=None, **opts):
     """``TensorNetwork2D.contract_boundary`` for labelled device arrays; see
     :class:`BoundaryContractor2D`.  Returns a Python scalar for a closed

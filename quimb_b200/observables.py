@@ -56,11 +56,11 @@ RDM_MAX_DIM = 64
 
 
 # ------------------------------------------------------------- the kernel ---
-def rdm_reduce(U, V):
+def rdm_reduce(U, V, out=None):
     """out[m, n] = sum_{a, b} U[a, m, b] conj(V[a, n, b]) through
     ``qb_rdm_reduce``: U (n1, M, n2) and V (n1, N, n2) torch tensors of one
     dtype, any strides; float32 / complex64 are widened, the result is fp64 /
-    c128 (M, N)."""
+    c128 (M, N), written into ``out`` (a contiguous (M, N) tensor) if given."""
     if U.dtype != V.dtype:
         raise TypeError(f"rdm_reduce: dtype mismatch {U.dtype} vs {V.dtype}")
     if U.dtype in _WIDE:
@@ -73,7 +73,10 @@ def rdm_reduce(U, V):
                          "in the summed extents")
     N = V.shape[1]
     lib = _lib.load()
-    out = torch.empty((M, N), dtype=U.dtype, device=U.device)
+    if out is None:
+        out = torch.empty((M, N), dtype=U.dtype, device=U.device)
+    elif out.shape != (M, N) or out.dtype != U.dtype or not out.is_contiguous():
+        raise ValueError(f"rdm_reduce: out must be a contiguous ({M}, {N}) {U.dtype} tensor")
     need = int(lib.qb_rdm_workspace(n1, M, N, n2))
     if need < 0:
         _lib.check(need, "qb_rdm_workspace")
