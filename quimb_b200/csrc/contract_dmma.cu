@@ -49,6 +49,11 @@ struct KernelCfg {
   static constexpr int B_ELEMS =
       (BN * (BK + 4) > BK * (BN + 4)) ? BN * (BK + 4) : BK * (BN + 4);
   static constexpr int BC_PITCH = BN / 2 + 2;  // complex elements
+  // A tile in k-pair layout (contract_tile, LA == 2): [k/2][row][2], the
+  // pairs of k of one row adjacent, pitch 2*BM+8 per pair of k (== 8 mod
+  // 16 doubles: fragment reads conflict free per half-warp, see load_af)
+  static constexpr int AP_PITCH = 2 * BM + 8;
+  static_assert(BK / 2 * AP_PITCH <= A_ELEMS, "k-pair A tile fits the stage");
   static constexpr size_t SMEM =
       (size_t)STAGES * (A_ELEMS + B_ELEMS) * 8       // tiles
       + (size_t)(2 * BM + 2 * BN) * 8                // m/n offset tables
@@ -150,7 +155,8 @@ struct AffineFeed {
   bool wide;  // 16-byte copies (vec != 0)
 };
 
-template <int ROWS, int BK, int NT, bool KMAJOR>
+// LAYOUT: 0 [k][row], 1 [row][k], 2 k pairs ([k/2][row][2], pitch PP)
+template <int ROWS, int BK, int NT, int LAYOUT, int PP = 0>
 __device__ __forceinline__ AffineFeed affine_setup(const double *base, int64_t rstep,
                                                    int64_t kstep, int vec, int thr,
                                                    int tid) {
@@ -163,7 +169,10 @@ __device__ __forceinline__ AffineFeed affine_setup(const double *base, int64_t r
   const int inner = thr ? BK / uk : ROWS / ur;
   const int a = tid % inner, b = tid / inner, db = NT / inner;
   const int ru = thr ? b : a, ku = thr ? a : b;
-  constexpr int s_row = KMAJOR ? BK + 4 : 1, s_k = KMAJOR ? 1 : ROWS + 4;
+  static_assert(LAYOUT != 2 || PP % 2 == 0, "k-pair layout: even pitch");
+  // (the k-pair layout takes 16-byte pairs of k, whose first k is even)
+  constexpr int s_row = LAYOUT == 1 ? BK + 4 : LAYOUT == 2 ? 2 : 1;
+  constexpr int s_k = LAYOUT == 1 ? 1 : LAYOUT == 2 ? PP / 2 : ROWS + 4;
   AffineFeed f;
   f.src = base + ru * rstep + ku * kstep;
   f.sm = (uint32_t)(ru * ur * s_row + ku * uk * s_k) * 8;
@@ -255,6 +264,8 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
   constexpr int NT = Cfg::NT;
   constexpr bool AFA = (FEED & 1) != 0, AFB = (FEED & 2) != 0;
   static_assert(FEED == 0 || (!CPLX && LA >= 0 && LB >= 0), "affine feed: real, fixed layout");
+  static_assert(LA != 2 || FEED == 3, "k-pair A tile: both operands affine");
+  static_assert(LB != 2, "k-pair layout: A tile only");
   constexpr int MT = Cfg::MT, NT8 = Cfg::NT8;
   constexpr int NCB = BN / 2, KCB = BK / 2;  // complex B tile extents
 
@@ -393,10 +404,10 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
   // affine operands: row 0 of the tile is in range (the planner proved
   // whole tiles), its table entry is the tile's base
   if constexpr (AFA)
-    fA = affine_setup<BM, BK, NT, LA == 1>(A + offAm[0] + kbeg / (p.vecA == 2 ? 2 : 1) * p.kstepA,
+    fA = affine_setup<BM, BK, NT, LA, Cfg::AP_PITCH>(A + offAm[0] + kbeg / (p.vecA == 2 ? 2 : 1) * p.kstepA,
                                            p.rstepA, p.kstepA, p.vecA, p.thrA, tid);
   if constexpr (AFB)
-    fB = affine_setup<BN, BK, NT, LB == 1>(B + offBn[0] + kbeg / (p.vecB == 2 ? 2 : 1) * p.kstepB,
+    fB = affine_setup<BN, BK, NT, LB>(B + offBn[0] + kbeg / (p.vecB == 2 ? 2 : 1) * p.kstepB,
                                            p.rstepB, p.kstepB, p.vecB, p.thrB, tid);
 #pragma unroll 1
   for (int s = 0; s < STAGES - 1; ++s) {
@@ -433,6 +444,19 @@ __device__ __forceinline__ void contract_tile(const ContractParams &p, int pid,
   // fragments of k-step kk: A row block i, B column block j
   auto load_af = [&](const double *tA, int kk, int i, double (&a)[4]) {
     const int r = wm0 + i * 16 + g;
+    if constexpr (LA == 2) {
+      // (r, k) at (k/2)*P + 2r + (k&1); kk is a multiple of 8, so k = kk+t
+      // is in pair kk/2 + t/2.  Per half-warp (g < 4 or g >= 4) lanes of
+      // t < 2 cover 8 consecutive doubles and lanes of t >= 2 the 8 that
+      // P == 8 mod 16 shifts them to: 16 distinct banks of 8 bytes
+      constexpr int P = Cfg::AP_PITCH;
+      const double *q = tA + 2 * r + (t >> 1) * P + (t & 1) + (kk / 2) * P;
+      a[0] = q[0];
+      a[1] = q[16];
+      a[2] = q[2 * P];
+      a[3] = q[2 * P + 16];
+      return;
+    }
     a[0] = tA[r * sAm + (kk + t) * sAk];
     a[1] = tA[(r + 8) * sAm + (kk + t) * sAk];
     a[2] = tA[r * sAm + (kk + t + 4) * sAk];
@@ -667,6 +691,18 @@ __global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
   classic_grid<BM, BN, BK, WARPS_M, WARPS_N, STAGES, false, LA, LB, FEED>(p);
 }
 
+// The large real tile with both operands affine and the A tile in k-pair
+// layout (LA == 2): for an A operand whose 16-byte pairs lie along k while
+// its threads walk rows (plan.h, a_kpair), e.g. an MPS site tensor read as
+// [b', (a', p)].  In [row][k] layout each 32-byte sector of a warp's
+// contiguous read lands in two rows 288 bytes apart; in k-pair layout a
+// sector is 32 contiguous bytes of the tile.  Same tile contents, same DMMAs
+template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES, int LB>
+__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
+    contract_f64_kpair_kernel(const __grid_constant__ ContractParams p) {
+  classic_grid<BM, BN, BK, WARPS_M, WARPS_N, STAGES, false, 2, LB, 3>(p);
+}
+
 // Stream-K: one persistent CTA per SM; the (tile, k-block) iteration space is
 // cut into gridDim.x equal contiguous ranges, so every SM gets the same number
 // of k-blocks whatever the tile count (no wave quantisation).  A range that
@@ -726,6 +762,12 @@ __global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
   streamk_grid<BM, BN, BK, WARPS_M, WARPS_N, STAGES, false, LA, LB, FEED>(p);
 }
 
+template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES, int LB>
+__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
+    contract_f64_kpair_streamk_kernel(const __grid_constant__ ContractParams p) {
+  streamk_grid<BM, BN, BK, WARPS_M, WARPS_N, STAGES, false, 2, LB, 3>(p);
+}
+
 // Stream-K pair schedule, for a stream-K grid with at most half as many tiles
 // as CTAs: the equal-cost cut is then "every tile in two halves".  The grid
 // runs as clusters of 2 CTAs; cluster c takes tile c (the same grouped
@@ -758,6 +800,12 @@ template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES, int LA,
 __global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
     contract_f64_affine_pair_kernel(const __grid_constant__ ContractParams p) {
   streamk_pair_grid<BM, BN, BK, WARPS_M, WARPS_N, STAGES, false, LA, LB, FEED>(p);
+}
+
+template <int BM, int BN, int BK, int WARPS_M, int WARPS_N, int STAGES, int LB>
+__global__ void __launch_bounds__(WARPS_M *WARPS_N * 32, 1)
+    contract_f64_kpair_pair_kernel(const __grid_constant__ ContractParams p) {
+  streamk_pair_grid<BM, BN, BK, WARPS_M, WARPS_N, STAGES, false, 2, LB, 3>(p);
 }
 
 // deterministic split-K reduction + strided scatter into C
@@ -839,6 +887,8 @@ static int launch_cfg(const ContractParams &p, cudaStream_t st) {
   auto kern = [] {
     if constexpr (FEED == 0)
       return contract_f64_kernel<BM, BN, BK, WARPS_M, WARPS_N, STAGES, CPLX, LA, LB>;
+    else if constexpr (LA == 2)
+      return contract_f64_kpair_kernel<BM, BN, BK, WARPS_M, WARPS_N, STAGES, LB>;
     else
       return contract_f64_affine_kernel<BM, BN, BK, WARPS_M, WARPS_N, STAGES, LA, LB, FEED>;
   }();
@@ -914,6 +964,8 @@ static int launch_pair_l(const PairPlan &plan, cudaStream_t st) {
   auto kern = [] {
     if constexpr (FEED == 0)
       return contract_f64_pair_kernel<128, 128, 32, 2, 4, 3, CPLX, LA, LB>;
+    else if constexpr (LA == 2)
+      return contract_f64_kpair_pair_kernel<128, 128, 32, 2, 4, 3, LB>;
     else
       return contract_f64_affine_pair_kernel<128, 128, 32, 2, 4, 3, LA, LB, FEED>;
   }();
@@ -933,6 +985,8 @@ static int launch_streamk_l(const PairPlan &plan, cudaStream_t st) {
   auto kern = [] {
     if constexpr (FEED == 0)
       return contract_f64_streamk_kernel<128, 128, 32, 2, 4, 3, CPLX, LA, LB>;
+    else if constexpr (LA == 2)
+      return contract_f64_kpair_streamk_kernel<128, 128, 32, 2, 4, 3, LB>;
     else
       return contract_f64_affine_streamk_kernel<128, 128, 32, 2, 4, 3, LA, LB, FEED>;
   }();
@@ -950,6 +1004,7 @@ static int launch_streamk_l(const PairPlan &plan, cudaStream_t st) {
 
 template <int LA, int LB>
 static int launch_streamk_feed(const PairPlan &plan, cudaStream_t st) {
+  if (LA == 1 && a_kpair(plan.p)) return launch_streamk_l<false, 2, LB, 3>(plan, st);
   switch (plan.p.feedA | plan.p.feedB << 1) {
     case 0: return launch_streamk_l<false, LA, LB, 0>(plan, st);
     case 1: return launch_streamk_l<false, LA, LB, 1>(plan, st);
@@ -974,6 +1029,7 @@ static int launch_streamk(const PairPlan &plan, const Route &r, cudaStream_t st)
 
 template <int LA, int LB>
 static int launch_cfg0_feed(const ContractParams &p, cudaStream_t st) {
+  if (LA == 1 && a_kpair(p)) return launch_cfg<128, 128, 32, 2, 4, 3, false, 2, LB, 3>(p, st);
   switch (p.feedA | p.feedB << 1) {
     case 0: return launch_cfg<128, 128, 32, 2, 4, 3, false, LA, LB, 0>(p, st);
     case 1: return launch_cfg<128, 128, 32, 2, 4, 3, false, LA, LB, 1>(p, st);

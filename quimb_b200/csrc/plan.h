@@ -444,6 +444,13 @@ inline int a_kmajor(const ContractParams &p) {
 inline int b_kmajor(const ContractParams &p) {
   return (p.vecB == 2) || (p.vecB == 0 && p.thrB == 1);
 }
+// the large real tile keeps A in k-pair layout ([k/2][row][2], contract_dmma.cu)
+// when both operands take the affine feed and A's 16-byte pairs of k are
+// gathered by threads that walk rows: each 32-byte sector a warp reads then
+// lands in 32 contiguous bytes of the tile rather than in two rows
+inline bool a_kpair(const ContractParams &p) {
+  return p.feedA && p.feedB && p.vecA == 2 && p.thrA == 0;
+}
 
 // Which kernel a contraction runs.  select_route (api.cu) decides the engine;
 // dmma_route fills in the DMMA details.  The launchers read the same fields,

@@ -10,6 +10,12 @@ its route (the stream-K grid is one CTA per SM).
 phases: 0 entry, 1 tables done, 2 prologue issued, 3 first tile landed,
         4 main loop done, 5 stream-K fix-up done (pair schedule: the
         distributed-shared-memory exchange of the two k-halves), 6 stores issued
+
+Each launch also reports its thread-block cluster shape (CTAs per cluster: 2
+for the stream-K pair schedule, 1 otherwise) and, where every CTA runs the
+same number of k-blocks (classic grid, pair schedule), the median main-loop
+time per k-block, to set against the DMMA issue rate of the 8-warp tile
+(DESIGN §5).
 """
 import ctypes
 import json
@@ -94,13 +100,22 @@ def main():
         f = qb.feed_pair(*args, ptrs=ptrs)
         r["schedule"] = qb.schedule_pair(*args, ptrs=ptrs)
         tiles = (x.shape[0] // 128) * (z.numel() // x.shape[0] // 128) if r["streamk"] == 0 else 0
-        grids.append((r["streamk"] or tiles, r, f))
+        K = int(np.prod([x.shape[i] for i, l in enumerate(lx) if l in ly and l not in lz]))
+        nkb = -(-K // r["bk"])
+        # k-blocks of one CTA: a classic CTA runs its split, a pair CTA one
+        # k-half; stream-K segments differ from CTA to CTA
+        kb_cta = {"pair": nkb / 2, None: nkb / r["splitk"]}.get(r["schedule"])
+        grids.append((r["streamk"] or tiles, r, f, 2 if r["schedule"] == "pair" else 1, kb_cta))
         print(json.dumps({"route": r, "feed": f}))
     res = []
     for n, i in enumerate(used):
-        G, r, f = grids[n % 2]
-        res.append({"kind": r["kind"], "layout": r["layout"], "ctas": G, "feed": f,
-                    "schedule": r["schedule"], **analyse(tr[i], G, r["schedule"])})
+        G, r, f, cluster, kb_cta = grids[n % 2]
+        a = analyse(tr[i], G, r["schedule"])
+        loop = a.get("seg0", {}).get("main_loop")
+        res.append({"kind": r["kind"], "layout": r["layout"], "ctas": G, "cluster": cluster,
+                    "feed": f, "schedule": r["schedule"], "kblocks_per_cta": kb_cta,
+                    "main_loop_us_per_kblock": round(loop / kb_cta, 3) if loop and kb_cta else None,
+                    **a})
     res.sort(key=lambda r: r["start_ns"])
     for k, r in enumerate(res):
         gap = (r["start_ns"] - res[k - 1]["end_ns"]) / 1e3 if k else None
